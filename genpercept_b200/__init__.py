@@ -1,4 +1,4 @@
-"""genpercept_b200 — B200-native (sm_100a) engine behind the GenPerceptPipeline API.
+"""genpercept_b200 — H100-native (sm_90a) engine behind the GenPerceptPipeline API.
 
 ``from genpercept_b200 import GenPerceptPipeline, GenPerceptOutput`` mirrors
 ``from genpercept import GenPerceptPipeline, GenPerceptOutput``

@@ -1,4 +1,4 @@
-"""Builds genpercept_b200/libgenpercept_b200.so in-tree with nvcc for sm_100a (no torch involved)."""
+"""Builds genpercept_b200/libgenpercept_b200.so in-tree with nvcc for sm_90a (no torch involved)."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["igemm.cu", "igemm_patch.cu", "fattn.cu", "kernels.cu", "imgproc.cu", "builder.cu", "engine.cu"]
 LIB = os.path.join(HERE, "libgenpercept_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -38,7 +38,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError("nvcc failed")
     if procs or not os.path.exists(LIB):
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs + ["-lcudart_static", "-lpthread", "-ldl", "-lrt"]
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + objs + ["-lcudart_static", "-lpthread", "-ldl", "-lrt"]
         subprocess.check_call(cmd)
     return LIB
 

@@ -108,30 +108,13 @@ void Builder::custom(const std::string& name, int launches, double bytes, std::f
 }
 
 static int ceil_div(int a, int b) { return (a + b - 1) / b; }
-static int choose_bn(int cout, int force) {
+// N tile: one of the wgmma widths the GEMM kernels are built for (16, 32, 64, 128).  Cout = 320 (the SD-2.1 UNet's first
+// level) takes 64 (five exact tiles): a multiple of 64 keeps the staged TMA-store epilogue.
+int choose_bn(int cout, int force) {
   if (force) return force;
-  const int c16 = ceil_div(cout, 16) * 16;
-  if (c16 <= 256) return c16;
-  // Cout = 320 / 640 (the SD-2.1 UNet's first two levels): an exact divisor (160) is not a multiple of 64 and forces the
-  // direct epilogue (16-byte stores at a 2*Cout-byte stride, per-thread residual rows, no GroupNorm statistics).  A
-  // multiple of 64 keeps the staged TMA-store epilogue even if the last N tile is partly empty: 640 = 5 x 128 exactly,
-  // 320 -> 2 x 192 (64 idle columns).  GP_BN_POLICY=0 restores the divisor rule (A/B switch).
-  static const int policy = std::getenv("GP_BN_POLICY") ? std::atoi(std::getenv("GP_BN_POLICY")) : 1;
-  if (policy && (cout % 64) == 0) {
-    for (int bn : {256, 192, 128})
-      if (cout % bn == 0) return bn;
-    if (policy == 2) return 128;
-    int best = 256, best_pad = 1 << 30;
-    for (int bn : {256, 192, 128}) {
-      const int pad = ceil_div(cout, bn) * bn - cout;
-      if (pad < best_pad) { best_pad = pad; best = bn; }
-    }
-    return best;
-  }
-  for (int bn = 256; bn >= 128; bn -= 16)
-    if (cout % bn == 0) return bn;
-  const int n = ceil_div(cout, 256);
-  return ceil_div(ceil_div(cout, n), 16) * 16;
+  for (int bn : {16, 32, 64})
+    if (cout <= bn) return bn;
+  return (cout % 128 == 0 || cout % 64 != 0) ? 128 : 64;
 }
 // pick the TW x TH = `rows` (128 or 256) patch with the least padding waste (ties: wider rows)
 static void choose_tile(int gw, int gh, int rows, int* tw, int* th, int* shift) {
@@ -146,12 +129,9 @@ static void choose_tile(int gw, int gh, int rows, int* tw, int* th, int* shift) 
 
 // Tile shape (BN, MT) for the layers that do not fill the GPU (the UNet's deep levels at any batch, everything at batch
 // 1).  Two bounds per candidate: the tensor time of the longest-running SM — ceil(tiles / SMs) waves of tiles whose
-// duration scales with the MMA width (a 128 x 64 x 16 MMA is bound by its 6 KB of operand fetch: 48 cycles, not 32) — and
-// the L2 -> SM operand traffic, tiles x K x (128 MT + BN) x 2 bytes at an effective 7 TB/s (what such few-tile layers sustain; r2n: the
-// 2560 -> 1280 conv on 8 x 12 x 12 pixels moves 796 MB with BN = 256 and 1062 MB with BN = 128: 152 vs 210 us, although
-// BN = 128 doubles the number of busy SMs; at batch 1 the same level has 2 M tiles, BN = 256 keeps 10 SMs busy for 61 us
-// and BN = 64 runs 40 tiles in ~25 us).  A candidate replaces the default only for a predicted gain above 10 %, so
-// every layer with many waves stays where choose_bn put it.  GP_TILE_MODEL=0: off (A/B switch).
+// duration scales with the MMA width (a narrow MMA is bound by its operand fetch) — and the L2 -> SM operand traffic,
+// tiles x K x (128 MT + BN) x 2 bytes.  A candidate replaces the default only for a predicted gain above 10 %, so every
+// layer with many waves stays where choose_bn put it.  GP_TILE_MODEL=0: off (A/B switch).
 struct TileShape { int bn, mt; };
 template <class MTilesFn>
 static TileShape choose_tile_shape(int cout, double k_elems, int num_sms, TileShape dflt, MTilesFn mtiles_of) {
@@ -168,9 +148,9 @@ static TileShape choose_tile_shape(int cout, double k_elems, int num_sms, TileSh
   TileShape best = dflt;
   const double c0 = cost(dflt);
   double best_cost = c0;
-  for (int bn : {256, 192, 128, 64})
+  for (int bn : {128, 64})
     for (int mt : {1, 2}) {
-      if (mt == 2 && bn > 128) continue;
+      if (mt == 2 && bn > 64) continue;
       const double c = cost(TileShape{bn, mt});
       if (c < 0.9 * c0 && c < best_cost) { best_cost = c; best = TileShape{bn, mt}; }
     }
@@ -182,7 +162,7 @@ static TileShape choose_tile_shape(int cout, double k_elems, int num_sms, TileSh
 void tile_shape_for(int cout, double k_elems, bool tokens_mode, int images, int gw, int gh, int num_sms, int* bn, int* mt) {
   const long long work_px = (long long)images * gw * gh;
   const int bn0 = choose_bn(cout, 0);
-  const int mt0 = (bn0 <= 128 && work_px >= 256LL * 148) ? 2 : 1;
+  const int mt0 = (bn0 <= 64 && work_px >= 256LL * num_sms) ? 2 : 1;
   auto mtiles_of = [&](int m) -> long long {
     if (tokens_mode) return (work_px + 128 * m - 1) / (128 * m);
     int tw = 128, th = m, sh = 7;
@@ -205,8 +185,7 @@ static void finalize_or_throw(IgemmParams* p, const std::string& name) {
 // The patch-resident kernel with the GroupNorm transform in its operand path (igemm_patch.cu) takes a convolution when:
 // 3x3 stride 1, ONE normalised source (channels % 64 == 0), at most one raw shortcut source, W % 128 == 0, and either the
 // staged epilogue (Cout % 64 == 0) or an fp32 map as output.  Opt-in (GP_GN_FUSE=1): it removes the GroupNorm passes over
-// the big maps (-8 ms, -38 GB of DRAM traffic per step) but its shared-memory traffic competes with the tensor core's own
-// operand fetch, which already uses the SM's whole shared-memory bandwidth on these layers: no net gain (DESIGN.md 4.1).
+// the big maps, but the transform runs inside the consumer warpgroup, between its wgmma batches.
 static bool gn_fusable(const ConvArgs& a, bool split) {
   const char* on = std::getenv("GP_GN_FUSE");        // read at plan time (tests toggle it)
   const bool off = on == nullptr || on[0] == '0' || std::getenv("GP_NO_PATCH") != nullptr;
@@ -261,7 +240,7 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   const long long work_px = tokens_mode ? (long long)N * H * W
                                         : (long long)(a.mode == 3 ? W : Wo) * (a.mode == 3 ? H : Ho) * N * (a.mode == 3 ? 4 : 1);
   int bn_pre = choose_bn(Cout, a.force_bn);
-  int mt_pre = gn_fused ? ((bn_pre <= 128 && (H % 2) == 0) ? 2 : 1) : (bn_pre <= 128 && work_px >= 256LL * 148) ? 2 : 1;
+  int mt_pre = (bn_pre <= 64 && work_px >= 256LL * num_sms) ? 2 : 1;
   if (!a.force_bn && !(a.flags & IG_GEGLU) && !gn_fused) {
     const double k_elems = flops / (2.0 * N * Ho * Wo * (double)Cout) * (a.mode == 3 ? 4.0 / 9.0 : 1.0);
     tile_shape_for(Cout, k_elems, tokens_mode, N * (a.mode == 3 ? 4 : 1), (a.mode == 3) ? W : Wo, (a.mode == 3) ? H : Ho, num_sms,
@@ -269,14 +248,20 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   }
   const bool is_geglu = (a.flags & IG_GEGLU) != 0;
   const bool staged = !a.out_f32 && std::getenv("GP_DIRECT_EPILOGUE") == nullptr &&
-                      (is_geglu ? (std::getenv("GP_STAGED_GEGLU") != nullptr && !split_ &&   // measured slower than the direct GEGLU stores (r1g)
+                      (is_geglu ? (std::getenv("GP_STAGED_GEGLU") != nullptr && !split_ &&   // opt-in: the direct GEGLU stores are the default
                                    Cout == 2 * a.out.C && (Cout % 128) == 0 && (bn_pre % 128) == 0)
                                 : (Cout == a.out.C && (Cout % 64) == 0 && (bn_pre % 64) == 0));
   // GP_STATS: 0 = never fuse the GroupNorm partial sums into conv epilogues, 1 = always (default), 2 = everywhere
   // except the patch-resident layers (whose main loop runs at the tensor-pipe limit, so the epilogue is critical)
   static const int stats_mode = std::getenv("GP_STATS") ? std::atoi(std::getenv("GP_STATS")) : 1;
-  const bool patch_eligible = gn_fused || (staged && a.mode == 0 && a.ks == 3 && a.srcs.size() == 1 && a.sc.empty() && mt_pre == 2 &&
-                                           (W % 128) == 0 && (H % 2) == 0 && !split_ && std::getenv("GP_NO_PATCH") == nullptr);
+  const bool patch_eligible = gn_fused || (staged && a.mode == 0 && a.ks == 3 && a.srcs.size() == 1 && a.sc.empty() &&
+                                           work_px >= 128LL * num_sms && (W % 128) == 0 && !split_ && std::getenv("GP_NO_PATCH") == nullptr);
+  // the patch-resident kernel takes one image row per tile and N tiles of 64: two 50 KiB halo patches, the weight ring and the
+  // 32 KiB accumulator tile fit in shared memory with the statistics scratch of any Cout <= 512
+  if (patch_eligible) {
+    bn_pre = 64;
+    mt_pre = 1;
+  }
   bool emit_stats = a.want_stats && staged && !is_geglu && Cout <= 512 && stats_mode != 0 && !(stats_mode == 2 && patch_eligible) && !split_;
   if (emit_stats && tokens_mode && ((long long)H * W) % (128 * mt_pre) != 0) emit_stats = false;
   size_t stats_off = 0;
@@ -529,7 +514,7 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
     p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
     p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = 1;
   };
-  if (d == 64 && !unfused && !split_) {   // fused tcgen05 flash-attention kernel (S and P stay on chip)
+  if (d == 64 && !unfused && !split_) {   // fused wgmma flash-attention kernel (S and P stay on chip)
     if (measuring_) return;
     FattnParams p;
     std::memset(&p, 0, sizeof(p));

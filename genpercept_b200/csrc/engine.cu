@@ -588,7 +588,7 @@ struct gp_engine {
     T4 gg = b.alloc(x.N, x.H, x.W, 4 * C);
     {
       ConvArgs c; c.srcs = {l3}; c.ks = 1; c.w = &packed.at(blk + ".ff.geglu_w"); c.out = gg; c.cout_valid = 8 * C;
-      c.flags = IG_GEGLU; c.force_bn = 256;
+      c.flags = IG_GEGLU; c.force_bn = 128;
       b.conv(blk + ".ff.proj_geglu", c);
     }
     b.release(l3);
@@ -1123,7 +1123,7 @@ gp_status gp_create(const gp_config* cfg, gp_engine** out) {
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= cfg->device) return GP_ERR_CUDA;
   if (cudaSetDevice(cfg->device) != cudaSuccess) return GP_ERR_CUDA;
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 10) return GP_ERR_CUDA;   // sm_100a only
+  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 9) return GP_ERR_CUDA;   // sm_90a only
   gp_engine* e = new gp_engine();
   e->cfg = *cfg;
   if (e->cfg.timestep <= 0) e->cfg.timestep = 1;
@@ -1297,8 +1297,7 @@ gp_status gp_infer(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host
       src = p->in_staging;
     }
     GP_CUDA(preprocess_rgb_im2col(src, kind, p->arena + p->kept["rgb"].t.off, p->B, p->H, p->W, e->bf16, s, e->split));
-    // 2 = auto: replay a graph where the launch stream is the bottleneck — small plans (measured: +15 % at 384x384,
-    // +8 % at 768x768 with one image, nothing at batch 8)
+    // 2 = auto: replay a graph where the launch stream is the bottleneck — small plans
     const bool use_graph = e->cfg.use_cuda_graph == 1 ||
                            (e->cfg.use_cuda_graph == 2 && (long long)p->B * p->H * p->W <= 2LL * 768 * 768);
     // eager launches write the result straight into a device `out`; a captured graph has the plan's own buffer baked in
@@ -1795,7 +1794,7 @@ gp_status gp_attention(int dtype, const void* q, const void* k, const void* v, i
       p.out = vT; p.outW = C; p.outH = 1; p.out_pix_stride = Tp; p.out_z1 = (long long)C * Tp;
       p.out_sy = p.out_sx = 1;
       p.Cout = T;
-      p.BN = (T + 15) / 16 * 16 <= 256 ? (T + 15) / 16 * 16 : 256;
+      p.BN = choose_bn(T, 0);
       GP_CUDA(make_tmap_a(&p.tmA[0], wv.w, wv.ktot, C, 1, 1, wv.ktot, (long long)C * wv.ktot, (long long)C * wv.ktot, 128, 1, te.e.bf16));
       for (int i = 1; i < 4; ++i) p.tmA[i] = p.tmA[0];
       GP_CUDA(make_tmap_b(&p.tmB, b.ptr(vin), C, T, B, C, (long long)T * C, p.BN, te.e.bf16));
@@ -1896,11 +1895,12 @@ gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int k
   });
 }
 
-/* debug (scripts/patch_trace.py): device buffer of >= 512 int64; CTA 0 of subsequent patch-kernel launches stamps clock64() per K chunk:
-   [i*8+0] transform starts waiting, +1 first patch row landed, +2 transform done; +4 MMA issuer starts waiting, +5 patch ready, +6 taps issued */
+/* debug: device buffer of >= 512 int64; CTA 0 of subsequent patch-kernel launches stamps clock64() per K chunk i < 60:
+   [i*8+4] consumer starts waiting for the patch, +5 patch ready (transformed if GroupNorm-fused), +6 all taps issued and retired */
 void gp_debug_patch_trace(void* dev_buf) { gp::igemm_patch_set_trace(reinterpret_cast<long long*>(dev_buf)); }
 
-/* debug: device buffer of >= 1024 int64 that CTA 0 of subsequently planned fused-attention launches fills with clock64() stamps */
+/* debug: device buffer of >= 512 int64 that CTA 0 of subsequently planned fused-attention launches fills with clock64() stamps
+   ([j*8+0] key block j starts, +1 S done, +2 P.V done; j < 64) */
 void gp_debug_fattn_trace(void* dev_buf) { gp::fattn_set_trace(reinterpret_cast<long long*>(dev_buf)); }
 
 }  // extern "C"

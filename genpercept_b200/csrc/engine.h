@@ -82,7 +82,7 @@ struct Op {
   int stage = 0;
   int variant = 0;            // 0: always; 1 / 3: only when out_channels matches
   int launches = 1;
-  int kind = 0;               // 1: tcgen05 implicit-GEMM launch, 0: anything else
+  int kind = 0;               // 1: wgmma implicit-GEMM launch, 2: fused attention, 0: anything else
   double flops = 0, bytes = 0;   // algorithmic work (SURVEY.md 8d): what the reference's op costs
   double flops_exec = -1;        // MMA work actually issued when it differs (upsample-fused convs run 4 of 9 taps); -1: = flops
   float usec = 0;
@@ -145,7 +145,7 @@ class Builder {
 
   struct StatsInfo { size_t off; int slots; int C; };
   std::map<long long, StatsInfo> stats;   // live tensors (by arena offset) whose producer emitted GN partial sums
-  int num_sms = 148;
+  int num_sms = 132;   // H100 SXM; replaced by the device's count at construction
 
   std::vector<Op> ops;
   int stage = 0;
@@ -168,6 +168,8 @@ class Builder {
 };
 
 // builder.cu: (BN, MT) of a stride-1 implicit-GEMM layer (default policy + the waves / L2-traffic model)
+// N tile width for a GEMM with `cout` output columns (`force` != 0: that width); one of 16, 32, 64, 128.
+int choose_bn(int cout, int force);
 void tile_shape_for(int cout, double k_elems, bool tokens_mode, int images, int gw, int gh, int num_sms, int* bn, int* mt);
 
 }  // namespace gp

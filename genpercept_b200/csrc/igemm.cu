@@ -1,22 +1,12 @@
-// tcgen05 implicit-GEMM kernel (see igemm.h for the operand model).
+// wgmma implicit-GEMM kernel (see igemm.h for the operand model).
 //
-// Warp roles (384 threads, 1 CTA / SM, persistent over a static round-robin tile list).  The single-thread
-// producer / issuer roles sit in the HIGHEST warp ids (8..11): the SM sub-partition arbiter favours higher warp
-// ids, and an issuer starved by the epilogue warps of its sub-partition stalls the tensor pipe (fattn trace, r1h).
-// Each single-thread role is executed by its WHOLE warp (every lane walks the loop and waits on the barriers) and
-// one elect.sync lane issues: coordinates and descriptors stay in uniform registers (back-to-back UTCHMMA).
-//   warp 8         : TMA producer A (activation box per 64-channel K block, `stages`-deep ring)
-//   warp 11        : TMA producer B (weight box per K block) — its own warp: one thread issuing
-//                    both boxes plus the barrier traffic could not keep up with BN=128 tiles
-//                    (ncu r1a: tensor pipe 45 % active on the 128->128 convs, DRAM/L2 not saturated)
-//   warp 9 (and 10): MMA issuer(s), one per accumulator tile (4 tcgen05.mma 128xBNx16 per K block; commit frees the slot)
-//   warp 10        : TMEM allocator (512 columns = 2 accumulator buffers x MT tiles)
-//   warps 0..7     : epilogue, two per sub-partition: warps w and w + 4 read the same TMEM lane quadrant and split the
-//                    tile's 64-channel groups (tcgen05.ld 32 lanes x 32 columns -> bias (from shared memory) / TMA-loaded
-//                    residual / act -> staged tile -> TMA store, GroupNorm partial sums from the staged tile).  One
-//                    epilogue warp per sub-partition was stalled 78 % of the time (ncu r2, the K = 1 stem GEMM).
-// MT = 2 (a 256-pixel M tile per CTA, two accumulators sharing every weight box) when BN <= 128:
-// halves the weight traffic and the per-byte barrier / TMA issue cost of the narrow-N layers.
+// Warp roles (384 threads, 1 CTA / SM, persistent over a static round-robin tile list; see igemm_common.cuh):
+//   warps 0..3  : epilogue (accumulator tile -> bias / residual / act -> staged tile -> TMA store, GroupNorm partial sums)
+//   warps 4..7  : wgmma consumer: per 64-channel K block, 4 x (MT * 2) wgmma m64 x BN x 16 from the stage's A and B boxes
+//   warp 8      : TMA producer A (activation box per 64-channel K block, `stages`-deep ring)
+//   warp 11     : TMA producer B (weight box per K block)
+// MT = 2 (a 256-pixel M tile per CTA sharing every weight box) when BN <= 64: the consumer holds MT * 128 x BN fp32
+// accumulators in registers, at most 128 per thread.
 #include "igemm.h"
 
 #include <cstdlib>
@@ -29,24 +19,75 @@ namespace gp {
 
 namespace {
 
-constexpr int kEpiWarps = 8;                         // epilogue warps 0..7; the single-thread roles are warps 8..11
-constexpr int kTapThreads = (kEpiWarps + 4) * 32;    // 384
+// K loop of the tap-streaming kernel for one (BN, MB = 2 * MT) instance; the whole consumer warpgroup runs it.
+template <bool BF16, int BN, int MB>
+__device__ __forceinline__ void tap_consumer(const IgemmParams& p, uint8_t* smem, int stage_bytes, int a_bytes, float* accs,
+                                             uint64_t* full_bar, uint64_t* empty_bar, uint64_t* tfull_bar, uint64_t* tempty_bar,
+                                             int wc, int lane) {
+  float d[MB][BN / 2];
+  int stage = 0;
+  uint32_t phase = 0, acc_phase = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const TileCoord t = decode_tile(p, tile);
+    const int cls = p.cls_from_z0 ? t.z0 : 0;
+    const int nkb = p.nkb[cls] * p.npass;
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait(&full_bar[stage], phase, 3);
+      const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
+      const uint64_t b_desc = make_sw128_kmajor_desc(a_addr + a_bytes);
+#pragma unroll
+      for (int mb = 0; mb < MB; ++mb) reg_fence(d[mb]);
+      wgmma_fence();
+#pragma unroll
+      for (int mb = 0; mb < MB; ++mb) {
+        const uint64_t a_desc = make_sw128_kmajor_desc(a_addr + mb * (kABytes / 2));
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k)   // +32 bytes per K step inside the 128-byte swizzle row -> +2 in the (addr >> 4) field
+          wgmma_ss<BN, BF16>(d[mb], a_desc + 2 * k, b_desc + 2 * k, (kb | k) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int mb = 0; mb < MB; ++mb) reg_fence(d[mb]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    }
+    mbar_wait(tempty_bar, acc_phase ^ 1, 2);     // the epilogue has read the previous tile
+    acc_store<BN, MB>(accs, p.acc_pitch, d, wc, lane);
+    mbar_arrive(tfull_bar);
+    acc_phase ^= 1;
+  }
+}
 
 template <bool BF16>
-__global__ void __launch_bounds__(kTapThreads, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
+__device__ __forceinline__ void run_tap_consumer(const IgemmParams& p, uint8_t* smem, int stage_bytes, int a_bytes, float* accs,
+                                                 uint64_t* full_bar, uint64_t* empty_bar, uint64_t* tfull_bar, uint64_t* tempty_bar,
+                                                 int wc, int lane) {
+#define GP_TAP(BN_, MB_) tap_consumer<BF16, BN_, MB_>(p, smem, stage_bytes, a_bytes, accs, full_bar, empty_bar, tfull_bar, tempty_bar, wc, lane)
+  if (p.MT == 2) {
+    if (p.BN == 16) GP_TAP(16, 4); else if (p.BN == 32) GP_TAP(32, 4); else GP_TAP(64, 4);
+  } else {
+    if (p.BN == 16) GP_TAP(16, 2); else if (p.BN == 32) GP_TAP(32, 2); else if (p.BN == 64) GP_TAP(64, 2); else GP_TAP(128, 2);
+  }
+#undef GP_TAP
+}
+
+template <bool BF16>
+__global__ void __launch_bounds__(kRoleThreads, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int a_bytes = kABytes * p.MT;
   const int stage_bytes = a_bytes + p.BN * 128;
   const int stages = p.stages;
   uint8_t* stg_base = smem + stages * stage_bytes;                     // one 4 KiB staging tile per epilogue warp (tma_store only)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + (p.tma_store ? (p.out_lo ? 2 : 1) * p.epi_warps * 4096 : 0));
+  float* accs = reinterpret_cast<float*>(stg_base + (p.tma_store ? (p.out_lo ? 2 : 1) * kEpiWarps * 4096 : 0));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(accs + 128 * p.MT * p.acc_pitch);
   uint64_t* empty_bar = full_bar + stages;
   uint64_t* tfull_bar = empty_bar + stages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* res_bar = tempty_bar + 2;                                  // [epilogue warps] residual tile landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + kEpiWarps);
-  float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 15) & ~uintptr_t(15));   // [kBiasSlots]
+  uint64_t* tempty_bar = tfull_bar + 1;
+  uint64_t* res_bar = tempty_bar + 1;                                  // [epilogue warps] residual tile landed
+  float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(res_bar + kEpiWarps) + 15) & ~uintptr_t(15));   // [bias_slots]
   float* sacc = sbias + p.bias_slots;   // [4 epilogue warps][Cout][2], only with p.stats
 
   const int warp = uniform_warp_id();
@@ -57,26 +98,20 @@ __global__ void __launch_bounds__(kTapThreads, 1) igemm_kernel(const __grid_cons
     tma_prefetch_desc(&p.tmB);
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 2);    // producer A + producer B
-      mbar_init(&empty_bar[i], p.MT);  // one tcgen05.commit per MMA issuer
+      mbar_init(&empty_bar[i], 4);   // the four consumer warps
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], p.MT);
-      mbar_init(&tempty_bar[i], p.epi_warps * 32);
-    }
+    mbar_init(tfull_bar, 128);
+    mbar_init(tempty_bar, kEpiWarps * 32);
     for (int i = 0; i < kEpiWarps; ++i) mbar_init(&res_bar[i], 1);
     fence_barrier_init();
   }
-  if (warp == kEpiWarps + 2) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_trigger();      // the next kernel of the stream may be scheduled (it blocks in its own pdl_wait until this grid is done)
-  pdl_wait();         // barriers / TMEM are set up; from here on the predecessor's outputs are read
+  pdl_wait();         // barriers are set up; from here on the predecessor's outputs are read
 
   // Single-thread roles run warp-uniform (every lane walks the loop and waits on the barriers) and one
-  // elected lane issues: the TMA coordinates / UMMA descriptors then stay in uniform registers.
-  if (warp == kEpiWarps) {
+  // elected lane issues: the TMA coordinates then stay in uniform registers.
+  if (warp == 8) {
     // ===================================================================== TMA producer A
     const bool leader = elect_one();
     int stage = 0;
@@ -106,7 +141,7 @@ __global__ void __launch_bounds__(kTapThreads, 1) igemm_kernel(const __grid_cons
         }
       }
     }
-  } else if (warp == kEpiWarps + 3) {
+  } else if (warp == 11) {
     // ===================================================================== TMA producer B
     const bool leader = elect_one();
     int stage = 0;
@@ -133,69 +168,18 @@ __global__ void __launch_bounds__(kTapThreads, 1) igemm_kernel(const __grid_cons
         }
       }
     }
-  } else if (warp == kEpiWarps + 1 || (warp == kEpiWarps + 2 && p.MT == 2)) {
-    const bool leader = elect_one();
-    // ===================================================================== MMA issuer(s)
-    // With two accumulator tiles (MT = 2, BN <= 128) each tile gets its own issuing thread: a single
-    // thread cannot issue one 64-cycle 128x128x16 MMA every 64 cycles once descriptor arithmetic and
-    // barrier polls are added (ncu r1h: tensor pipe 57 % busy, issuer never blocked on a barrier).
-    const uint32_t idesc = make_idesc_f16(kBM, p.BN, BF16 ? 1 : 0);
-    const int h_lo = warp - (kEpiWarps + 1), h_hi = (p.MT == 2) ? warp - kEpiWarps : 1;
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const TileCoord t = decode_tile(p, tile);
-      const int cls = p.cls_from_z0 ? t.z0 : 0;
-      const int nkb = p.nkb[cls] * p.npass;
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1, 2);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * kAccStride;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&full_bar[stage], phase, 3);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-        const uint64_t b_desc = make_sw128_kmajor_desc(a_addr + a_bytes);
-        if (leader) {
-          for (int h = h_lo; h < h_hi; ++h) {
-            const uint64_t a_desc = make_sw128_kmajor_desc(a_addr + h * kABytes);
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k) {
-              // +32 bytes per UMMA_K inside the 128-byte swizzle row -> +2 in the (addr >> 4) field
-              umma_f16(d_tmem + h * 128, a_desc + 2 * k, b_desc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-        }
-        __syncwarp();
-        if (++stage == stages) { stage = 0; phase ^= 1; }
-      }
-      if (leader) umma_commit(&tfull_bar[acc]);
-      __syncwarp();
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  } else if (warp < kEpiWarps && p.epi_warps == kEpiWarps) {
-    if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
-    else run_epilogue_direct<BF16, kEpiWarps>(p, sacc, sbias, tfull_bar, tempty_bar, tmem_base, warp, lane);
-  } else if (warp < 4) {
-    // four epilogue warps (warps 4..7 idle): the long-K BN = 256 layers, where eight 4 KiB staging tiles would cost the fourth
-    // pipeline stage (igemm_finalize) and the epilogue is hidden behind an 18 k-cycle main loop anyway
-    if (p.tma_store) run_epilogue_staged<BF16, 4, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
-    else run_epilogue_direct<BF16, 4>(p, sacc, sbias, tfull_bar, tempty_bar, tmem_base, warp, lane);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kEpiWarps + 2) {
-    __syncwarp();          // reconverge before the .aligned dealloc
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+  } else if (warp >= kConsumerWarp0 && warp < kConsumerWarp0 + 4) {
+    // ===================================================================== wgmma consumer
+    run_tap_consumer<BF16>(p, smem, stage_bytes, a_bytes, accs, full_bar, empty_bar, tfull_bar, tempty_bar, warp - kConsumerWarp0, lane);
+  } else if (warp < kEpiWarps) {
+    if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+    else run_epilogue_direct<BF16, kEpiWarps>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
   }
 }
 
-// ------------------------------------------------------------------------------------------------
+}  // namespace
+
+namespace {
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
@@ -248,8 +232,10 @@ cudaError_t make_tmap_b(CUtensorMap* m, const void* base, long long K, long long
   return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
+static int acc_tile_bytes(const IgemmParams& p) { return 128 * p.MT * p.acc_pitch * (int)sizeof(float); }
+
 size_t igemm_smem_bytes(const IgemmParams& p) {
-  return (size_t)p.stages * (kABytes * p.MT + p.BN * 128) + (2 * p.stages + 4) * 8 + 16 + 1024;
+  return (size_t)p.stages * (kABytes * p.MT + p.BN * 128) + acc_tile_bytes(p) + (2 * p.stages + 6) * 8 + 16 + 1024;
 }
 
 const char* igemm_finalize(IgemmParams* p) {
@@ -260,11 +246,11 @@ const char* igemm_finalize(IgemmParams* p) {
   if (p->out_lo && (p->stats || p->res_tma || p->patch || (p->flags & IG_OUT_F32_NCHW)))
     return "the high-precision output layout excludes epilogue statistics, TMA residuals, the patch loop and fp32 maps";
   if (p->MT != 1 && p->MT != 2) return "MT must be 1 or 2";
-  if (p->MT == 2 && p->BN > 128) return "MT=2 needs BN <= 128 (TMEM: 2 buffers x 2 tiles x BN columns)";
+  if (p->BN != 16 && p->BN != 32 && p->BN != 64 && p->BN != 128) return "BN must be 16, 32, 64 or 128";
+  if (p->MT == 2 && p->BN > 64) return "MT=2 needs BN <= 64 (the consumer holds at most 128 x 128 accumulators per warpgroup)";
   if (p->TW * p->TH != kBM * p->MT) return "TW*TH must be 128*MT";
   if (p->TW > 256 || p->TH > 256) return "TMA box dims are limited to 256";
   if ((1 << p->tw_shift) != p->TW) return "TW must be a power of two";
-  if (p->BN < 16 || p->BN > 256 || (p->BN % 16)) return "BN must be a multiple of 16 in [16,256]";
   if (p->Z0 < 1 || p->Z1 < 1) return "bad batch dims";
   p->tiles_x = (p->gridW + p->TW - 1) / p->TW;
   p->tiles_y = (p->gridH + p->TH - 1) / p->TH;
@@ -281,60 +267,35 @@ const char* igemm_finalize(IgemmParams* p) {
   long long total = (long long)p->n_tiles_n * p->tiles_x * p->tiles_y * p->Z0 * p->Z1;
   if (total > 0x7fffffffLL) return "too many tiles";
   p->total_tiles = (int)total;
-  const int stage_bytes = kABytes * p->MT + p->BN * 128;
   const int stats_bytes = p->stats ? 4 * p->Cout * 2 * (int)sizeof(float) : 0;
   if (p->tma_store && ((p->Cout % 64) || (p->BN % 64) || (p->flags & IG_OUT_F32_NCHW) || p->out_z0 != 0))
     return "staged epilogue needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output";
   if (p->tma_store && (p->flags & IG_GEGLU) && ((p->Cout % 128) || (p->BN % 128))) return "staged GEGLU needs Cout, BN % 128 == 0";
   if (p->stats && (!p->tma_store || p->Cout > 512 || (p->flags & IG_GEGLU))) return "statistics need the staged epilogue and Cout <= 512";
-  // staging: one 4 KiB tile per epilogue warp (8; 4 in the patch kernel's GroupNorm-transform build), x2 for the (hi, lo) layout
-  int epi_warps = (p->patch && p->gn_ss) ? 4 : 8;
-  // patch-resident layers without a residual: four warps and the fourth 16 KiB weight-ring stage (see igemm_patch.cu, NE4)
-  if (p->patch && !p->gn_ss && p->tma_store && !p->res_tma && p->res1 == nullptr && p->res2 == nullptr && getenv("GP_PATCH_NE8") == nullptr)
-    epi_warps = 4;
-  auto staging_of = [&](int ew) { return p->tma_store ? ew * 4096 * (p->out_lo ? 2 : 1) : 0; };
-  int nkb_max = 0;
-  for (int c = 0; c < ncls; ++c) nkb_max = p->nkb[c] > nkb_max ? p->nkb[c] : nkb_max;
-  // Eight staging tiles + the statistics scratch leave the BN = 256 layers three 48 KiB stages instead of four (r2: the
-  // 512- and 256-channel VAE convs ran 8-15 % slower than in round 1: 929 -> 1006..1069 us).  Their main loop is >= 16 K
-  // blocks (18 k cycles per tile) and hides a four-warp epilogue, so those layers keep four warps and the fourth stage.
-  if (!p->patch && epi_warps == 8 && nkb_max >= 16 && getenv("GP_EPI_WARPS8") == nullptr &&
-      (kMaxSmem - 3072 - stats_bytes - staging_of(4)) / stage_bytes > (kMaxSmem - 3072 - stats_bytes - staging_of(8)) / stage_bytes)
-    epi_warps = 4;
-  p->epi_warps = epi_warps;
-  const int staging = staging_of(epi_warps);
-  // bias: one N tile (288 floats, inside the 3072 reserved bytes) or the whole padded vector when it is small (<= 16 KiB)
-  p->bias_slots = kBiasSlots;
-  p->bias_all = 0;
-  if (p->n_tiles_n > 1 && p->n_tiles_n * p->BN + 32 <= 4096 && getenv("GP_NO_BIAS_ALL") == nullptr) {
-    p->bias_all = 1;
-    p->bias_slots = p->n_tiles_n * p->BN + 32;
-  }
-  int bias_extra = (p->bias_slots - kBiasSlots) * (int)sizeof(float);
-  int st = (kMaxSmem - 3072 - stats_bytes - staging - bias_extra) / stage_bytes;
-  // ... but never at the price of a pipeline stage: the BN = 256 layers fit exactly four 48 KiB stages, and the UNet's deep
-  // levels (L2-latency-bound) lost 25-30 % with three (r2r: 2560 -> 1280 on 8 x 12 x 12 pixels 134 -> 179 us)
-  if (p->bias_all && !p->patch && st < (kMaxSmem - 3072 - stats_bytes - staging) / stage_bytes) {
-    p->bias_all = 0;
-    p->bias_slots = kBiasSlots;
-    bias_extra = 0;
-    st = (kMaxSmem - 3072 - stats_bytes - staging) / stage_bytes;
-  }
+  p->epi_warps = kEpiWarps;
+  p->acc_pitch = (p->BN + 31) & ~31;
+  // fixed part: staging (one 4 KiB tile per epilogue warp, x2 for the (hi, lo) layout), the accumulator tile, 3 KiB for
+  // barriers and one N tile of bias, the statistics scratch
+  const int fixed = (p->tma_store ? kEpiWarps * 4096 * (p->out_lo ? 2 : 1) : 0) + acc_tile_bytes(*p) + 3072 + stats_bytes;
+  const int ring_unit = p->patch ? p->BN * 128 : kABytes * p->MT + p->BN * 128;   // bytes per pipeline stage
   if (p->patch) {
     if (p->TW != 128 || p->TH != p->MT || p->Z0 != 1 || p->Z1 < 1 || p->nseg[0] != 9 + (p->kc_sc > 0 ? 1 : 0) || p->kc_count < 1 ||
         p->nkb[0] != 9 * p->kc_count + p->kc_sc || p->npass != 1 || p->gridW % 128 || p->gridH % p->TH)
       return "patch mode needs TW = 128, TH = MT, full tiles and a single-source 3x3 tap table (+ shortcut chunks)";
     if (p->gn_ss && p->gn_C != p->kc_count * 64) return "patch mode: GroupNorm channels must equal the source's";
     p->a_slot_bytes = ((p->TW + 2) * (p->TH + 2) * 128 + 1023) & ~1023;
-    st = (kMaxSmem - 3072 - stats_bytes - staging - bias_extra - 2 * p->a_slot_bytes) / (p->BN * 128);
-    if (p->bias_all && st < (kMaxSmem - 3072 - stats_bytes - staging - 2 * p->a_slot_bytes) / (p->BN * 128)) {
-      p->bias_all = 0;
-      p->bias_slots = kBiasSlots;
-      st = (kMaxSmem - 3072 - stats_bytes - staging - 2 * p->a_slot_bytes) / (p->BN * 128);
-    }
-    if (const char* env = getenv("GP_PATCH_STAGES")) {          // experiment: depth of the weight ring
-      const int v = atoi(env);
-      if (v >= 2 && v < st) st = v;
+  }
+  const int avail = kMaxSmem - 1024 - fixed - (p->patch ? 2 * p->a_slot_bytes : 0);
+  int st = avail / ring_unit;
+  // bias: one N tile (288 floats, inside the 3 KiB) or, when the layer has several N tiles, the whole padded vector (<= 16 KiB),
+  // loaded once instead of on every change of tile column, unless that costs a pipeline stage
+  p->bias_slots = kBiasSlots;
+  p->bias_all = 0;
+  if (p->n_tiles_n > 1 && p->n_tiles_n * p->BN + 32 <= 4096 && getenv("GP_NO_BIAS_ALL") == nullptr) {
+    const int extra = (p->n_tiles_n * p->BN + 32 - kBiasSlots) * (int)sizeof(float);
+    if ((avail - extra) / ring_unit == st) {
+      p->bias_all = 1;
+      p->bias_slots = p->n_tiles_n * p->BN + 32;
     }
   }
   if (st > 8) st = 8;
@@ -375,13 +336,13 @@ cudaError_t igemm_launch(const IgemmParams& p, cudaStream_t stream) {
   if (p.total_tiles <= 0) return cudaSuccess;
   if (p.stats && p.stats_slots < (p.total_tiles < g_num_sms ? p.total_tiles : g_num_sms)) return cudaErrorInvalidValue;
   const int grid = p.total_tiles < g_num_sms ? p.total_tiles : g_num_sms;
-  // always request the maximum so exactly one CTA (512 TMEM columns) is resident per SM
+  // always request the maximum so exactly one CTA is resident per SM
   const size_t smem = kMaxSmem;
   if (p.patch) return igemm_patch_launch(p, grid, stream);
   if (p.flags & IG_BF16) {
-    launch(igemm_kernel<true>, grid, kTapThreads, smem, stream, p);
+    launch(igemm_kernel<true>, grid, kRoleThreads, smem, stream, p);
   } else {
-    launch(igemm_kernel<false>, grid, kTapThreads, smem, stream, p);
+    launch(igemm_kernel<false>, grid, kRoleThreads, smem, stream, p);
   }
   return cudaGetLastError();
 }

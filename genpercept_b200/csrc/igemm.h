@@ -1,4 +1,4 @@
-// Persistent warp-specialised tcgen05 implicit-GEMM: the one tensor-core kernel behind every 3x3
+// Persistent warp-specialised wgmma implicit-GEMM: the one tensor-core kernel behind every 3x3
 // convolution (stride 1, stride 2, nearest-2x-upsample-fused), 1x1 convolution / linear layer
 // and batched attention GEMM of the hot path.
 //
@@ -8,8 +8,8 @@
 // 128-row M tile is a TW x TH spatial patch, loaded per K-chunk of 64 channels as one TMA box whose
 // start coordinate carries the filter-tap offset (halo/padding = TMA out-of-bounds zero fill).
 // B operand: K-major [rows, K] matrix (packed weights, or activations for attention), 3-D map.
-// Accumulators: fp32 in TMEM, double buffered (2 x 256 columns) so the epilogue of tile i overlaps
-// the main loop of tile i+1.
+// Accumulators: fp32 in the consumer warpgroup's registers during the K loop, then handed to the epilogue warps
+// through an fp32 tile in shared memory, so the epilogue of tile i overlaps the main loop of tile i+1.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -19,7 +19,7 @@ namespace gp {
 
 constexpr int kMaxSegs = 20;
 constexpr int kMaxClasses = 4;
-constexpr int kBM = 128;      // UMMA M (TMEM lanes)
+constexpr int kBM = 128;      // rows of one accumulator tile (two wgmma m64 blocks)
 constexpr int kBK = 64;       // channels per pipeline stage (= one 128-byte swizzle row of fp16)
 
 struct IgemmSeg {
@@ -42,7 +42,7 @@ struct IgemmParams {
   CUtensorMap tmB;
   CUtensorMap tmB2;              // lo plane of an ACTIVATION B operand (attention GEMMs, high-precision mode)
   // High-precision mode (gp_config::precision = 1): every operand is an fp16 (hi, lo) pair and the K loop runs
-  // three passes over the segment table, accumulating hi*hi + lo*hi + hi*lo in the same fp32 TMEM accumulator.
+  // three passes over the segment table, accumulating hi*hi + lo*hi + hi*lo in the same fp32 accumulator.
   // Packed weights carry both planes along K: [.. ktot hi .. | .. ktot lo ..].
   int npass;                     // 1, or 3
   int pass_amap[3];              // added to IgemmSeg::map          {0, 4, 0}
@@ -56,7 +56,7 @@ struct IgemmParams {
   int nkb[kMaxClasses];          // total K blocks per class
   int8_t cls_py[kMaxClasses], cls_px[kMaxClasses];
   int out_sy, out_sx;            // output pixel = tile-grid pixel * s + (py, px)
-  int MT;                        // 128-row accumulator tiles per CTA tile: 1, or 2 when BN <= 128
+  int MT;                        // 128-row accumulator tiles per CTA tile: 1, or 2 when BN <= 64
   int TW, TH, tw_shift;          // M tile = TH rows x TW cols, TW*TH == 128*MT, TW = 1 << tw_shift
   int tiles_x, tiles_y, n_tiles_n, BN;
   int gridW, gridH;              // valid extent of the tile grid (pixels)
@@ -90,12 +90,13 @@ struct IgemmParams {
   CUtensorMap tmOut[kMaxClasses];   // (C, W, H, N) views of the output, box (64, min(TW,32), 32/min(TW,32), 1)
   // Residual through TMA (staged epilogue, res1 only): the same boxes of the residual tensor are LOADED into the
   // staging tile before the accumulator is read.  Row-per-thread global loads of a residual cost 32 L1 sector
-  // look-ups per warp request (ncu r1k: 58 % tensor pipe with a residual vs 92 % without, same layer).
+  // look-ups per warp request.
   int res_tma;
   int bias_slots;                // floats of shared memory holding the bias: 288 (one N tile, reloaded per tile) or, when the
                                  // layer has several N tiles and Cout is small enough, all of them (loaded once: bias_all)
   int bias_all;
-  int epi_warps;                 // epilogue warps of the tap-streaming kernel: 8, or 4 where 8 would cost a pipeline stage (igemm_finalize)
+  int epi_warps;                 // epilogue warps (4: warps 0..3)
+  int acc_pitch;                 // floats per row of the shared accumulator tile (BN rounded up to 32)
   int res_prefetch;              // L2-prefetch the next tile's residual boxes one tile period ahead (GP_NO_RES_PREFETCH=1: off)
   CUtensorMap tmRes[kMaxClasses];
   // Patch-resident main loop (igemm_patch.cu; 3x3 stride-1, one source, TW = 128, TH = MT = 1 or 2): per
@@ -111,7 +112,7 @@ struct IgemmParams {
   CUtensorMap tmPatch2;          // same box over the shortcut source
   // GroupNorm(+SiLU) of the patch source applied in shared memory before the MMA reads it (patch mode only):
   // y = silu(x * scale + shift), (scale, shift) = gn_ss[(image * gn_C + channel) * 2 + {0, 1}] (gn_finalize's output).
-  long long* trace;              // debug (gp_debug_patch_trace): CTA 0 stamps clock64() per K chunk; null = off
+  long long* trace;              // debug (gp_debug_patch_trace): CTA 0 stamps clock64() at slots 8k+4..8k+6 of K chunk k; null = off
   const float* gn_ss;            // null: the source is used as it is
   int gn_C;                      // channels of the normalised tensor (= the patch source's)
   int gn_silu;

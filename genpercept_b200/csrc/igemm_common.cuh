@@ -1,5 +1,10 @@
-// Device code shared by the two tcgen05 implicit-GEMM kernels (tap-streaming: igemm.cu, patch-resident:
-// igemm_patch.cu): tile decoding, 16-bit helpers, the exact-erf GELU and the two epilogues.
+// Device code shared by the two wgmma implicit-GEMM kernels (tap-streaming: igemm.cu, patch-resident:
+// igemm_patch.cu): tile decoding, 16-bit helpers, the exact-erf GELU, the accumulator hand-off and the two epilogues.
+//
+// Both kernels run three warpgroups (384 threads, 1 CTA / SM): warps 0..3 epilogue, warps 4..7 the wgmma consumer
+// (its fp32 accumulators live in registers during the K loop), warps 8..11 TMA producers.  At the end of a tile the
+// consumer writes its accumulators into an fp32 tile in shared memory and starts the next tile's K loop while the
+// epilogue warps read that tile one row per thread (tfull / tempty: single buffer, the registers are the second one).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -11,9 +16,10 @@ namespace gp {
 namespace {
 
 constexpr int kABytes = kBM * kBK * 2;       // 16 KiB per 128-row tile
-constexpr int kTmemCols = 512;
-constexpr int kAccStride = 256;              // TMEM columns between the two accumulator buffers
 constexpr int kMaxSmem = 227 * 1024;
+constexpr int kEpiWarps = 4;                 // warps 0..3
+constexpr int kConsumerWarp0 = 4;            // warps 4..7: the wgmma warpgroup
+constexpr int kRoleThreads = 384;
 
 struct TileCoord {
   int n_tile, tx, ty, z0, z1;
@@ -80,9 +86,51 @@ __device__ __forceinline__ void store8_hl(uint16_t* op, long long lo, const floa
   }
 }
 
+// ---------------------------------------------------------------- accumulator tile in shared memory
+// fp32 [128 * MT rows][acc_pitch], acc_pitch = BN rounded up to 32; the 16-byte chunks of a row are XOR-swizzled by
+// (row & 7) so that a warp reading eight consecutive rows one row per thread hits eight different bank groups.
+__device__ __forceinline__ int acc_chunk(int ch, int row) { return (ch & ~7) | ((ch ^ row) & 7); }
+
+// row `row`, columns c .. c + N - 1 (N = 16 or 32, c % 16 == 0) -> r[0 .. N-1]
+template <int N>
+__device__ __forceinline__ void acc_ld(const float* accs, int pitch, int row, int c, uint32_t (&r)[32]) {
+  const float* rp = accs + (size_t)row * pitch;
+#pragma unroll
+  for (int q = 0; q < N / 4; ++q) {
+    const float4 v = *reinterpret_cast<const float4*>(rp + (acc_chunk((c >> 2) + q, row) << 2));
+    r[4 * q] = __float_as_uint(v.x); r[4 * q + 1] = __float_as_uint(v.y);
+    r[4 * q + 2] = __float_as_uint(v.z); r[4 * q + 3] = __float_as_uint(v.w);
+  }
+}
+
+template <int BN, bool BF16>
+__device__ __forceinline__ void wgmma_ss(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (BN == 16) wgmma_ss_n16<BF16>(d, a, b, acc);
+  else if constexpr (BN == 32) wgmma_ss_n32<BF16>(d, a, b, acc);
+  else if constexpr (BN == 64) wgmma_ss_n64<BF16>(d, a, b, acc);
+  else wgmma_ss_n128<BF16>(d, a, b, acc);
+}
+
+// The consumer's register accumulators (MB m64 blocks: tile rows 64 mb ..) -> the shared tile.  wc: warp in the warpgroup.
+template <int BN, int MB>
+__device__ __forceinline__ void acc_store(float* accs, int pitch, float (&d)[MB][BN / 2], int wc, int lane) {
+#pragma unroll
+  for (int mb = 0; mb < MB; ++mb) {
+    reg_fence(d[mb]);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = 64 * mb + 16 * wc + (lane >> 2) + 8 * hh, col = 8 * j + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(accs + (size_t)row * pitch + (acc_chunk(col >> 2, row) << 2) + (col & 3)) =
+            make_float2(d[mb][4 * j + 2 * hh], d[mb][4 * j + 2 * hh + 1]);
+      }
+  }
+}
+
 // gelu(g) = g * Phi(g), exact-erf form (what diffusers' GEGLU uses), with erf from Abramowitz-Stegun 7.1.26
 // (|error| <= 1.5e-7): one MUFU.RCP, one MUFU.EX2 and a degree-5 Horner instead of erff()'s two-branch
-// polynomial — the GEGLU projection is bound by its epilogue (tensor pipe 33 %, ncu r1_final).
+// polynomial — the GEGLU projection is bound by its epilogue.
 //   1 - erf(z) = (a1 t + ... + a5 t^5) e^{-z^2},  t = 1 / (1 + p z),  z = |g| / sqrt(2)
 __device__ __forceinline__ float gelu_erf(float g) {
   const float z = fabsf(g) * 0.70710678118654752f;
@@ -98,18 +146,16 @@ __device__ __forceinline__ float gelu_erf(float g) {
   return g * (g >= 0.f ? 1.f - q : q);
 }
 
-// NW epilogue warps (4 or 8).  With 8, warps w and w + 4 read the same TMEM lane quadrant (lanes 32 * (w % 4) ...) and split the
-// tile's 64-channel groups between them: one epilogue warp per sub-partition is stalled ~78 % of the time (TMEM / shared
-// memory latency, instruction fetch: ncu r2, the K = 1 stem GEMM), a second one fills those slots.
+// NW epilogue warps (4 or 8).  With 8, warps w and w + 4 read the same accumulator rows (32 * (w % 4) ...) and split the
+// tile's 64-channel groups between them.
 template <int NW>
 __device__ __forceinline__ void epi_sync() {   // the epilogue threads only
   asm volatile("bar.sync 1, %0;" ::"n"(NW * 32) : "memory");
 }
 
 // The bias of the CTA's current N tile lives in shared memory (kBiasSlots floats, zero beyond Cout): every 32-column piece
-// of the epilogue used to fetch it with eight dependent 16-byte global loads — with almost all of L1 configured as shared
-// memory those miss to L2 (~600 cycles), in front of every piece (ncu r2: the K = 1 stem GEMM, nothing but epilogue, ran
-// with the epilogue warps issuing 22 % of the time and no unit above 25 %).
+// of the epilogue would otherwise fetch it with eight dependent 16-byte global loads — with almost all of L1 configured as
+// shared memory those miss to L2, in front of every piece.
 constexpr int kBiasSlots = 288;
 // A layer with several N tiles changes tile column on every tile of a CTA (tiles are numbered N-fastest and taken with a
 // stride of gridDim.x), i.e. two barriers of all epilogue warps plus an L2 round trip per tile: when the padded Cout fits
@@ -132,21 +178,20 @@ __device__ __forceinline__ void bias32(const float* sbias, int c, float (&bz)[32
   }
 }
 
-// Staged epilogue (shared by the tap-streaming and the patch-resident main loops): TMEM -> registers
+// Staged epilogue (shared by the tap-streaming and the patch-resident main loops): accumulator tile -> registers
 // (bias / residuals / ReLU) -> 16-bit rows in a SWIZZLE_128B shared tile -> one TMA store per
 // (warp, 64-channel group), plus the GroupNorm partial sums read back column-wise from the tile.
-// SPLIT / RES / GEGLU are compile-time: with run-time flags one 32 x 64 piece executed ~830 warp instructions, 97 of them MOVs
-// and 27 branches around the variants not taken (ncu source page, r2q: the 320 -> 2560 linear issues 13.4 k warp
-// instructions per 128 x 256 tile against 2560 tensor cycles).  RES: 0 none, 1 residual tile through TMA, 2 per-thread rows.
+// SPLIT / RES / GEGLU are compile-time: with run-time flags every 32 x 64 piece pays the moves and branches around the
+// variants not taken.  RES: 0 none, 1 residual tile through TMA, 2 per-thread rows.
 template <bool BF16, int NW, bool SPLIT, int RES, bool GEGLU>
 __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* stg_base, float* sacc, float* sbias, uint64_t* tfull_bar,
-                                                uint64_t* tempty_bar, uint64_t* res_bar, uint32_t tmem_base, int warp, int lane) {
+                                                uint64_t* tempty_bar, uint64_t* res_bar, const float* accs, int warp, int lane) {
   // ===================================================================== epilogue, staged + TMA store
-  // TMEM -> registers (bias / residuals / ReLU) -> 16-bit rows in a SWIZZLE_128B shared tile ->
+  // accumulator tile -> registers (bias / residuals / ReLU) -> 16-bit rows in a SWIZZLE_128B shared tile ->
   // one TMA store per (warp, 64-channel group): full-line writes instead of 16-byte pieces at a
   // 2C-byte stride, and image-edge clipping for free.  GroupNorm partial sums are read back
   // column-wise from the staged tile (conflict-free), in a fixed order.
-  const int wq = warp & 3;                   // epilogue warps are warps 0..NW-1; warp % 4 -> TMEM lanes [32*wq, +32)
+  const int wq = warp & 3;                   // epilogue warps are warps 0..NW-1; warp % 4 -> tile rows [32*wq, +32)
   const int half = warp >> 2;                // NW == 8: which of the tile's 64-channel groups this warp takes (parity)
   uint8_t* stg = stg_base + warp * 4096;
   const uint32_t stg_addr = smem_u32(stg);
@@ -159,7 +204,6 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
   const bool two_groups = NW == 8 && (p.BN >> gshift) >= 2;
   auto mine = [&](int c0) { return NW == 4 || (two_groups ? ((c0 >> gshift) & 1) == half : half == 0); };
   const int sw = lane & 7;
-  int acc = 0;
   uint32_t acc_phase = 0, res_phase = 0;
   const bool relu = (p.flags & IG_RELU) != 0;
   constexpr bool geglu = GEGLU;
@@ -193,9 +237,8 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
     }
     const int bias_origin = p.bias_all ? 0 : n_base;
     // The residual boxes of this CTA's NEXT tile are pulled into L2 now, a whole tile period before their TMA loads:
-    // those loads sit serially in front of every 32 x 64 piece of the epilogue, and with DRAM latency (1.5 us under
-    // load) four of them per warp outlast the main loop of the short-K (Cout = 128) layers (r2: residual convs 20-30 %
-    // slower than plain ones; the main loop of a 128->128 tile is 6 us).
+    // those loads sit serially in front of every 32 x 64 piece of the epilogue, and at DRAM latency under load four of
+    // them per warp can outlast the main loop of the short-K (Cout = 128) layers.
     if (RES == 1 && p.res_prefetch && lane == 0 && tile + (int)gridDim.x < p.total_tiles) {
       const TileCoord tn = decode_tile(p, tile + gridDim.x);
       const int ncls = p.cls_from_z0 ? tn.z0 : 0;
@@ -222,7 +265,6 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
       const int oy = gy * p.out_sy + p.cls_py[cls], ox = gx * p.out_sx + p.cls_px[cls];
       const long long pix_off = t.z1 * p.out_z1 + (long long)oy * p.out_row_stride + (long long)ox * p.out_pix_stride;
       const int sx = t.tx * p.TW + (r0 & (p.TW - 1)), sy = t.ty * p.TH + (r0 >> p.tw_shift);   // store box origin
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * kAccStride + h * 128;
       for (int c0 = 0; c0 < p.BN; c0 += 64) {
         const int n0 = n_base + c0;
         if (n0 >= p.Cout) break;
@@ -237,13 +279,11 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
             float bz[32];
             bias32(sbias, ns - bias_origin, bz);
             if (!waited) {
-              mbar_wait(&tfull_bar[acc], acc_phase, 4);
-              tc_fence_after();
+              mbar_wait(tfull_bar, acc_phase, 4);
               waited = true;
             }
             uint32_t r[32];
-            tmem_ld_32x32(taddr + c0 + sub * 32, r);
-            tmem_ld_wait();
+            acc_ld<32>(accs, p.acc_pitch, row, c0 + sub * 32, r);
             float g[16];
 #pragma unroll
             for (int q = 0; q < 16; ++q) {
@@ -307,13 +347,11 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
             for (int q = 0; q < 4; ++q) r2[q] = rp[q];
           }
           if (!waited) {
-            mbar_wait(&tfull_bar[acc], acc_phase, 4);
-            tc_fence_after();
+            mbar_wait(tfull_bar, acc_phase, 4);
             waited = true;
           }
           uint32_t r[32];
-          tmem_ld_32x32(taddr + c0 + sub * 32, r);
-          tmem_ld_wait();
+          acc_ld<32>(accs, p.acc_pitch, row, c0 + sub * 32, r);
           float v[32];
 #pragma unroll
           for (int q = 0; q < 32; ++q) v[q] = __uint_as_float(r[q]) + bz[q];
@@ -388,13 +426,10 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
       }
     }
     if (!waited) {
-      mbar_wait(&tfull_bar[acc], acc_phase, 4);
-      tc_fence_after();
+      mbar_wait(tfull_bar, acc_phase, 4);
     }
-    tc_fence_before();
-    mbar_arrive(&tempty_bar[acc]);
-    acc ^= 1;
-    if (acc == 0) acc_phase ^= 1;
+    mbar_arrive(tempty_bar);
+    acc_phase ^= 1;
   }
   if (lane == 0) tma_store_wait_read0();
   if (do_stats && cur_img >= 0) flush_stats(cur_img);
@@ -404,36 +439,35 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
 // Run-time flags -> the specialised staged epilogue.  LEAN (the patch-resident kernel): no (hi, lo) layout, no GEGLU.
 template <bool BF16, int NW, bool LEAN>
 __device__ __forceinline__ void run_epilogue_staged(const IgemmParams& p, uint8_t* stg_base, float* sacc, float* sbias, uint64_t* tfull_bar,
-                                                    uint64_t* tempty_bar, uint64_t* res_bar, uint32_t tmem_base, int warp, int lane) {
+                                                    uint64_t* tempty_bar, uint64_t* res_bar, const float* accs, int warp, int lane) {
   const int rm = p.res_tma ? 1 : ((p.res1 != nullptr || p.res2 != nullptr) ? 2 : 0);
   if constexpr (!LEAN) {
     if (p.flags & IG_GEGLU) {
-      epilogue_staged<BF16, NW, false, 0, true>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
+      epilogue_staged<BF16, NW, false, 0, true>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
       return;
     }
     if (p.out_lo != 0) {
-      if (rm == 2) epilogue_staged<BF16, NW, true, 2, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
-      else epilogue_staged<BF16, NW, true, 0, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
+      if (rm == 2) epilogue_staged<BF16, NW, true, 2, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+      else epilogue_staged<BF16, NW, true, 0, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
       return;
     }
   }
-  if (rm == 1) epilogue_staged<BF16, NW, false, 1, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
-  else if (rm == 2) epilogue_staged<BF16, NW, false, 2, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
-  else epilogue_staged<BF16, NW, false, 0, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, tmem_base, warp, lane);
+  if (rm == 1) epilogue_staged<BF16, NW, false, 1, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+  else if (rm == 2) epilogue_staged<BF16, NW, false, 2, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+  else epilogue_staged<BF16, NW, false, 0, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
 }
 
-// Direct epilogue: TMEM -> registers (bias / residuals / ReLU / affine clamp / GEGLU) -> global stores straight from
+// Direct epilogue: accumulator tile -> registers (bias / residuals / ReLU / affine clamp / GEGLU) -> global stores straight from
 // the registers: fp32 NCHW maps, odd channel counts, GEGLU, the high-precision (hi, lo) layout.
 // LEAN = the GEGLU projection of the default mode (full 32-column chunks, no residual, 16-bit output, no (hi, lo) planes): every
 // other variant is compiled out of its loop (same reasoning as the staged epilogue's template parameters).
 template <bool BF16, int NW, bool LEAN>
 __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sacc, float* sbias, uint64_t* tfull_bar, uint64_t* tempty_bar,
-                                                uint32_t tmem_base, int warp, int lane) {
+                                                const float* accs, int warp, int lane) {
   // ===================================================================== epilogue
-  const int wq = warp & 3;                 // warp % 4 -> TMEM lanes [32*wq, 32*wq+32)
+  const int wq = warp & 3;                 // warp % 4 -> tile rows [32*wq, 32*wq+32)
   const int half = warp >> 2;              // NW == 8: the tile's 32-column chunks go to the two halves by parity
   const bool two_chunks = NW == 8 && p.BN > 32;
-  int acc = 0;
   uint32_t acc_phase = 0;
   const bool f32out = !LEAN && (p.flags & IG_OUT_F32_NCHW) != 0;
   const bool relu = !LEAN && (p.flags & IG_RELU) != 0;
@@ -487,7 +521,6 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sac
       const int oy = gy * p.out_sy + p.cls_py[cls], ox = gx * p.out_sx + p.cls_px[cls];
       const long long pix_off = t.z1 * p.out_z1 + t.z0 * p.out_z0 + (long long)oy * p.out_row_stride +
                                 (long long)ox * p.out_pix_stride;
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * kAccStride + h * 128;
       for (int c0 = 0; c0 < p.BN; c0 += 32) {
         if (NW == 8 && (two_chunks ? ((c0 >> 5) & 1) != half : half != 0)) continue;
         const int ncols = (LEAN || p.BN - c0 >= 32) ? 32 : 16;
@@ -512,13 +545,11 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sac
           for (int q = 0; q < 4; ++q) if (q * 8 < ncols) r2[q] = rp[q];
         }
         if (!waited) {
-          mbar_wait(&tfull_bar[acc], acc_phase, 4);
-          tc_fence_after();
+          mbar_wait(tfull_bar, acc_phase, 4);
           waited = true;
         }
         uint32_t r[32];
-        if (LEAN || ncols == 32) tmem_ld_32x32(taddr + c0, r); else tmem_ld_32x16(taddr + c0, r);
-        tmem_ld_wait();
+        if (LEAN || ncols == 32) acc_ld<32>(accs, p.acc_pitch, row, c0, r); else acc_ld<16>(accs, p.acc_pitch, row, c0, r);
         if (!live) continue;
         float v[32];
 #pragma unroll
@@ -599,24 +630,21 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sac
       }
     }
     if (!waited) {   // unreachable (BN >= 16), kept so the barrier protocol can never desynchronise
-      mbar_wait(&tfull_bar[acc], acc_phase, 4);
-      tc_fence_after();
+      mbar_wait(tfull_bar, acc_phase, 4);
     }
-    tc_fence_before();
-    mbar_arrive(&tempty_bar[acc]);
-    acc ^= 1;
-    if (acc == 0) acc_phase ^= 1;
+    mbar_arrive(tempty_bar);
+    acc_phase ^= 1;
   }
   if (do_stats && cur_img >= 0) flush_stats(cur_img);
 }
 
 template <bool BF16, int NW>
 __device__ __forceinline__ void run_epilogue_direct(const IgemmParams& p, float* sacc, float* sbias, uint64_t* tfull_bar,
-                                                    uint64_t* tempty_bar, uint32_t tmem_base, int warp, int lane) {
+                                                    uint64_t* tempty_bar, const float* accs, int warp, int lane) {
   const bool lean = (p.flags & IG_GEGLU) && !(p.flags & (IG_OUT_F32_NCHW | IG_RELU | IG_AFFINE_CLAMP01)) && p.out_lo == 0 &&
                     p.res1 == nullptr && p.res2 == nullptr && (p.BN % 32) == 0 && (p.Cout % p.BN) == 0;
-  if (lean) epilogue_direct<BF16, NW, true>(p, sacc, sbias, tfull_bar, tempty_bar, tmem_base, warp, lane);
-  else epilogue_direct<BF16, NW, false>(p, sacc, sbias, tfull_bar, tempty_bar, tmem_base, warp, lane);
+  if (lean) epilogue_direct<BF16, NW, true>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
+  else epilogue_direct<BF16, NW, false>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
 }
 
 }  // namespace

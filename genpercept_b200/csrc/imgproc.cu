@@ -196,7 +196,7 @@ __global__ void quantize_kernel(const float* __restrict__ pred, void* __restrict
 }
 
 int grid_for(long long n, int dev) {
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long b = (n + 255) / 256;
   const long long cap = (long long)sms * 8;               // a multiple of the SM count; grid-stride loops cover the rest

@@ -40,7 +40,7 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 }
 // SiLU with ONE special-function op per element: x*sigmoid(x) = h + h*tanh(h), h = x/2.  tanh.approx.f32 has
 // ~2^-11 relative error, i.e. below the fp16 rounding of the stored result; exp + reciprocal (2 MUFU ops
-// per element) made the normalise+SiLU pass special-function-bound at 16 ops/clk/SM (r1d).
+// per element) would make the normalise+SiLU pass special-function-bound.
 __device__ __forceinline__ float silu_f(float x) {
   const float h = 0.5f * x;
   float t;
@@ -192,8 +192,8 @@ __global__ void gn_stats_kernel(const uint16_t* __restrict__ x, long long HW, in
 
 // One CTA of 256 threads per (image, group): the partial sums (one slot per producing CTA or pixel chunk, up to
 // 256 x channels-per-group entries) are read with all 8 warps in flight and reduced in a fixed order (thread ->
-// warp shuffle -> 8 warp totals), so the result does not depend on scheduling.  (One WARP per group left the
-// kernel latency-bound on 32 SMs: 113 launches x 16 us = 1.8 ms of a 95 ms step, ncu r1_final.)
+// warp shuffle -> 8 warp totals), so the result does not depend on scheduling.  (One WARP per group would leave the
+// kernel latency-bound on the few SMs that have a group.)
 __global__ void __launch_bounds__(256) gn_finalize_kernel(GnSrc s0, GnSrc s1, int nsrc, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, int N, int Ctot, int groups,
                                                           float inv_count, float eps, float* __restrict__ ss) {
@@ -292,7 +292,7 @@ __global__ void gn_apply_kernel(const uint16_t* __restrict__ x, long long HW, in
 // ------------------------------------------------------------------------------ LayerNorm
 constexpr int kLnMaxVec = 5;   // C <= 1280
 // One warp per token; KV = 8-channel vectors per lane (2 for C <= 512, 3 for C <= 768, 5 for C <= 1280).  Sized to
-// the channel count the kernel keeps ~35 registers at C = 320 instead of 64 (r1_final: 1.2 TB/s at half occupancy).
+// the channel count the kernel keeps ~35 registers at C = 320 instead of 64 (full occupancy for the narrow layers).
 template <bool BF16, int KV, int TOK>
 __global__ void __launch_bounds__(256) layernorm_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, long long tokens,
                                                         int C, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -382,7 +382,7 @@ __global__ void softmax_rows_small_kernel(uint16_t* __restrict__ s, long long ro
 }
 
 // MV = 8-column vectors per thread: 8 (any T up to 16384, 256 threads) or 3 with 512 threads for T <= 12288 — the
-// VAE mid-block rows (T = 9216) then hold 24 values per thread instead of 64 (r1_final: 2.5 TB/s at low occupancy).
+// VAE mid-block rows (T = 9216) then hold 24 values per thread instead of 64 (higher occupancy).
 template <bool BF16, int MV>
 __global__ void softmax_rows_kernel(uint16_t* __restrict__ s, int T, int Tp, int lo) {
   pdl_trigger();
@@ -436,8 +436,8 @@ __global__ void softmax_rows_kernel(uint16_t* __restrict__ s, int T, int Tp, int
 // Long rows (the VAE mid-block attention, T = 9216: 18 KiB per row, 73 728 rows per step and attention): a persistent
 // CTA streams its rows through a 3-slot shared-memory ring with bulk async copies — slot k + 2 is loading and slot
 // k - 1 is draining to global memory while row k is reduced in registers — so each SM keeps several rows in flight in
-// both directions.  The one-row-per-CTA kernel above has its loads, two block reductions and stores back to back
-// (r2: 2.4 TB/s, 1.1 ms per attention; this one is bound by the copy rate).
+// both directions.  The one-row-per-CTA kernel above has its loads, two block reductions and stores back to back;
+// this one is bound by the copy rate.
 constexpr int kSmPipeThreads = 384;
 constexpr int kSmPipeSlots = 3;
 template <bool BF16, int MV>
@@ -636,7 +636,7 @@ __global__ void xattn2_kernel(const uint16_t* __restrict__ x, uint16_t* __restri
 
 // Same operator with the folded weights resident in shared memory.  The kernel above re-reads U and M (2 * heads * C
 // floats: 12.8 / 51 / 205 KB at C = 320 / 640 / 1280) through L1 for every warp's tokens — 0.94 GB of L2 traffic per
-// launch at every level, 100-160 us for a 6-94 MB activation (r2 per-op events).  Here a persistent CTA loads them once,
+// launch at every level.  Here a persistent CTA loads them once,
 // its warps loop over token groups, and the heads are taken five at a time so that the five warp reductions and
 // sigmoids of a batch are independent chains instead of one serial chain per head.
 constexpr int kXaHB = 5;
@@ -656,7 +656,7 @@ __global__ void __launch_bounds__(KV >= 5 ? 512 : 256) xattn2_smem_kernel(const 
     const int n4 = heads * C / 4;
     const float4* gU = reinterpret_cast<const float4*>(U);
     const float4* gM = reinterpret_cast<const float4*>(M);
-    // four loads of each matrix in flight per thread (one per iteration left the 205 KB fill of C = 1280 latency-bound: 25 us)
+    // four loads of each matrix in flight per thread (one per iteration leaves the 205 KB fill of C = 1280 latency-bound)
     int i = threadIdx.x;
     for (; i + 3 * (int)blockDim.x < n4; i += 4 * blockDim.x) {
       float4 a[4], b[4];
@@ -860,7 +860,7 @@ __global__ void preprocess_kernel(const void* __restrict__ in, int kind, uint16_
 // K-packed stem: the 3x3 neighbourhood of every pixel laid out along the channel axis, NHWC32 =
 // [centre tap (3 ch) | the other 8 taps in row-major order (24 ch) | 5 zeros], so that AutoencoderKL.encoder.conv_in
 // (3 -> 128, 3x3) becomes a 1x1 GEMM with K = 27 (one 64-channel chunk) instead of nine 64-wide chunks of which 3
-// channels are real (1177 us -> one pass bound by the 1.2 GB output write at 8 x 768^2).  Out-of-image taps are zero.
+// channels are real (one pass bound by the output write).  Out-of-image taps are zero.
 template <bool BF16>
 __global__ void preprocess_im2col_kernel(const void* __restrict__ in, int kind, uint16_t* __restrict__ out, int N, int H, int W,
                                          int lo) {
@@ -936,7 +936,7 @@ __global__ void minmax_apply_kernel(float* __restrict__ x, long long HW, const u
     x[(long long)n * HW + i] = (x[(long long)n * HW + i] - mn) / d;
 }
 
-inline int blocks_for(long long total, int threads, int cap = 148 * 16) {
+inline int blocks_for(long long total, int threads, int cap = 132 * 16) {
   long long b = (total + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
@@ -1007,8 +1007,6 @@ cudaError_t gn_apply(const void* x, int N, long long HW, int C, const float* ss,
   int pix = 256 / nvec;
   if (pix < 1) pix = 1;
   if (pix > 32) pix = 32;
-  // (a software-pipelined variant — next four loads in flight during the arithmetic, 72 registers — and 4x longer pixel
-  //  strips per block measured 97.9 / 98.0 ms per step against 96.3-96.9 for this form, r2o)
   const int pix_per_block = pix * 16;
   dim3 block(nvec, pix);
   dim3 grid((unsigned)((HW + pix_per_block - 1) / pix_per_block), N);
@@ -1029,7 +1027,7 @@ cudaError_t layernorm(const void* x, void* y, long long tokens, int C, const flo
   const uint16_t* xi = reinterpret_cast<const uint16_t*>(x);
   uint16_t* yo = reinterpret_cast<uint16_t*>(y);
   const int kv = (C / 8 + 31) / 32;
-  // one token per warp; two per warp (all loads up front) measured slower: 80 registers, 0.87 -> 1.08 ms per step (r2m)
+  // one token per warp
   const int tok = 1;
   const long long blocks = (tokens + tpb * tok - 1) / (tpb * tok);
   if (kv <= 2)

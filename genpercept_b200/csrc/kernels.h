@@ -1,7 +1,7 @@
 // Bandwidth-bound and small kernels of the hot path (everything that is not a dense contraction):
 // GroupNorm(+SiLU), LayerNorm, row softmax, the 2-token cross-attention closed form, GEGLU,
 // ReLU, bilinear 2x, direct convolution for tiny channel counts (and as the on-device triage
-// reference for the tcgen05 kernel), pre/post-processing.  16-bit NHWC activations, fp32 math.
+// reference for the wgmma kernels), pre/post-processing.  16-bit NHWC activations, fp32 math.
 // `split` = the high-precision layout: C logical channels stored as [hi C | lo C] per pixel (two fp16 planes,
 // value = hi + lo); rows of score matrices as [hi Tp | lo Tp].
 #pragma once

@@ -1,7 +1,6 @@
 // Kernel launch helper: cudaLaunchKernelEx, optionally with the programmatic-dependent-launch attribute (see ptx.cuh,
-// pdl_wait).  Opt-in (GP_PDL=1): measured in one call (r2m) it changed nothing at batch 8 (95.05 / 96.21 ms with, 94.98 ms
-// without) and cost 1-2 % at batch 1 (384^2 .. 1024^2: 8.99 / 10.65 / 15.68 / 26.71 ms with, 8.84 / 10.45 / 15.59 / 26.54 ms
-// without) — inside a CUDA graph the launch gaps are already ~1 us and the early-resident CTAs only add scheduling work.
+// pdl_wait).  Opt-in (GP_PDL=1): inside a CUDA graph the launch gaps are already short and the early-resident CTAs
+// only add scheduling work.
 #pragma once
 #include <cuda_runtime.h>
 

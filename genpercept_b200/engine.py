@@ -106,7 +106,7 @@ class Engine:
     def __init__(self, dtype=torch.float16, readout="vae", timestep=1, device=0, cuda_graph="auto",
                  precision="default", arch="genpercept"):
         if not torch.cuda.is_available():
-            raise RuntimeError("genpercept_b200 needs a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("genpercept_b200 needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.L = lib()
         self.torch_dtype = dtype
         self.readout = readout
@@ -119,7 +119,7 @@ class Engine:
         self.h = c_void_p()
         st = self.L.gp_create(byref(cfg), byref(self.h))
         if st != 0:
-            raise RuntimeError(f"gp_create failed: {_STATUS.get(st, st)} (no sm_100a device?)")
+            raise RuntimeError(f"gp_create failed: {_STATUS.get(st, st)} (no sm_90a device?)")
         self.plan_shape = None
         self.out_hw = None
 
@@ -430,8 +430,8 @@ def quantize(pred, bits=16, to_host=True):
     return out
 
 
-def tile_shape(cout, cin, ks, images, h, w, tokens_mode=False, num_sms=148):
-    """(BN, MT) the planner gives a stride-1 layer (host-only, DESIGN.md section 4 "Tile shape per layer")."""
+def tile_shape(cout, cin, ks, images, h, w, tokens_mode=False, num_sms=132):
+    """(BN, MT) the planner gives a stride-1 layer (host-only; the rule is tile_shape_for in csrc/builder.cu)."""
     bn, mt = c_int(), c_int()
     st = lib().gp_tile_shape(cout, cin, ks, images, h, w, 1 if tokens_mode else 0, num_sms, byref(bn), byref(mt))
     _check_free(st, "gp_tile_shape")

@@ -1,4 +1,4 @@
-/* genpercept_b200 — C-ABI of the B200-native one-step perception engine.
+/* genpercept_b200 — C-ABI of the H100-native one-step perception engine.
  *
  * This is the drop-in boundary for the hot path of aim-uofa/GenPercept:
  *   GenPerceptPipeline.single_infer        /root/reference/genpercept/genpercept_pipeline.py:375-486
@@ -7,7 +7,7 @@
  *     decode_pred (/0.18215, post_quant_conv, vae.decoder, channel mean)       :507-526
  *     clip(-1,1), (x+1)/2                                                      :470-472
  *     or the DPT readout (customized_head on multi_level_feats, min-max)       :475-482
- * Everything below the boundary is hand-written sm_100a CUDA; there is no CPU fallback: every
+ * Everything below the boundary is hand-written sm_90a CUDA; there is no CPU fallback: every
  * entry point returns GP_ERR_CUDA when no CUDA device / kernel image is available.
  *
  * Plain C types only.  Device pointers are raw CUdeviceptr-compatible addresses (e.g.
@@ -80,7 +80,7 @@ int gp_plan_count(gp_engine* e);
 /* Host-only introspection (no device needed): the N tile (BN) and the number of 128-pixel M tiles per CTA (MT) the planner
  * gives a stride-1 ks x ks convolution / linear layer cin -> cout over `images` maps of h x w output pixels on a GPU with
  * num_sms SMs (tokens_mode != 0: one row of images * h * w tokens).  Nothing in the reference corresponds to it (PyTorch /
- * cuDNN pick their own tiles); it pins the tile policy of DESIGN.md section 4 in the CPU tests. */
+ * cuDNN pick their own tiles); it pins the tile policy of tile_shape_for (csrc/builder.cu) in the CPU tests. */
 gp_status gp_tile_shape(int cout, int cin, int ks, int images, int h, int w, int tokens_mode, int num_sms, int* bn, int* mt);
 /* replaces: the per-call `fix_timesteps` of single_infer (/root/reference/genpercept/genpercept_pipeline.py:405-408).
  * The timestep only enters through conv1.bias + time_emb_proj(silu(emb(t))) of the 22 UNet ResNets; those biases are
@@ -128,13 +128,13 @@ gp_status gp_plan_info(gp_engine* e, int64_t* n_ops, int64_t* n_kernel_launches,
                        int64_t* weight_bytes, double* igemm_flops);
 /* name/us of the i-th op after gp_profile_ops ran the plan once with CUDA events per op. */
 gp_status gp_profile_ops(gp_engine* e, int out_channels, void* stream);
-/* kind: 1 = tcgen05 implicit-GEMM launch, 2 = fused attention, 0 = other kernels.  flops = algorithmic work of the op
+/* kind: 1 = wgmma implicit-GEMM launch, 2 = fused attention, 0 = other kernels.  flops = algorithmic work of the op
  * (SURVEY.md 8d); flops_exec = MMA work actually issued (differs for the upsample-fused convolutions: 4 of 9 taps). */
 gp_status gp_op_info(gp_engine* e, int64_t i, char* name_buf, size_t name_cap, double* usec, double* flops,
                      double* bytes, int* kind, double* flops_exec);
 
 /* ---- per-kernel entry points (parity tests, micro-benchmarks); all pointers are device ---- */
-/* 3x3 / 1x1 convolution through the tcgen05 implicit-GEMM kernel.  x: 16-bit NHWC [N,H,W,Cin];
+/* 3x3 / 1x1 convolution through the wgmma implicit-GEMM kernels.  x: 16-bit NHWC [N,H,W,Cin];
  * w: fp32 [Cout,Cin,ks,ks] (host); mode: 0 stride-1 pad ks/2, 1 stride-2 pad (1,1,1,1),
  * 2 stride-2 pad (0,1,0,1) (VAE encoder), 3 nearest-2x upsample then stride-1.  y: 16-bit NHWC. */
 gp_status gp_conv2d(int dtype, const void* x, int N, int H, int W, int Cin, const float* w_host,
@@ -183,12 +183,13 @@ gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, v
 /* time one igemm configuration: returns average microseconds over `iters` launches */
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters,
                         double* usec, double* flops);
-/* debug (scripts/fattn_trace.py): a device buffer of >= 1024 int64 that CTA 0 of the fused-attention launches planned
- * afterwards fills with clock64() stamps at its phase boundaries; NULL switches the stamps off again. */
+/* debug: a device buffer of >= 512 int64 that CTA 0 of the fused-attention launches planned afterwards fills with
+ * clock64() stamps, slots 8j + {0, 1, 2} of key block j < 64: block start, S = Q K^T done, O += P V done (thread 0);
+ * NULL switches the stamps off again. */
 void gp_debug_fattn_trace(void* dev_buf);
-/* debug (scripts/patch_trace.py): a device buffer of >= 512 int64 that CTA 0 of the patch-resident kernel launches made
- * afterwards fills with clock64() stamps per K chunk (transform: wait / first row landed / done; MMA issuer: wait / ready /
- * issued); NULL switches the stamps off. */
+/* debug: a device buffer of >= 512 int64 that CTA 0 of the patch-resident kernel launches made afterwards fills with
+ * clock64() stamps, slots 8k + {4, 5, 6} of K chunk k < 60 (wgmma consumer: before the patch wait / patch ready, after
+ * the GroupNorm transform if any / all taps issued and retired); NULL switches the stamps off. */
 void gp_debug_patch_trace(void* dev_buf);
 
 #ifdef __cplusplus

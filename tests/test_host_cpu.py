@@ -96,19 +96,21 @@ def test_dropin_seeds_the_reference_import_path(tmp_path):
 
 
 def test_tile_shape_policy():
-    """The planner's (BN, MT) table (DESIGN.md section 4): many-wave layers keep the wide default, layers that do not fill the
+    """The planner's (BN, MT) table (tile_shape_for in csrc/builder.cu): many-wave layers keep the wide default, layers that do not fill the
     GPU get narrower N tiles only where the L2 operand traffic allows (host-only C-ABI entry, no device needed)."""
     from genpercept_b200 import engine as E
-    # big VAE layers: untouched by the model
-    assert E.tile_shape(128, 128, 3, 8, 768, 768) == (128, 2)
-    assert E.tile_shape(256, 256, 3, 8, 384, 384) == (256, 1)
-    assert E.tile_shape(512, 512, 3, 8, 192, 192) == (256, 1)
-    # Cout = 320 / 640: multiples of 64 (staged epilogue), never the divisor 160
-    assert E.tile_shape(320, 960, 3, 8, 96, 96)[0] in (192, 128)
-    assert E.tile_shape(640, 640, 3, 8, 48, 48) == (128, 2)            # 48 x 48 level at batch 8: two M tiles (fewer weight re-reads)
-    # batch 8, 12 x 12 level, 2560 -> 1280: stays at BN = 256 (narrower tiles would move more bytes through L2: measured 152 vs 210 us)
-    assert E.tile_shape(1280, 2560, 3, 8, 12, 12) == (256, 1)
-    # batch 1, same level: 10 of 148 SMs busy with BN = 256 -> narrow N tiles
+    # big VAE layers: untouched by the model (N tiles are at most 128 wide: the wgmma consumer holds 128 x 128 accumulators).
+    # These 3x3 layers over W % 128 == 0 maps then run in the patch-resident kernel, which replaces the planner's shape with
+    # (64, 1) (Builder::conv): one image row of halo patch, N tiles of 64.
+    assert E.tile_shape(128, 128, 3, 8, 768, 768) == (128, 1)
+    assert E.tile_shape(256, 256, 3, 8, 384, 384) == (128, 1)
+    assert E.tile_shape(512, 512, 3, 8, 192, 192) == (128, 1)
+    # Cout = 320: a multiple of 64 (staged epilogue), never the divisor 160; wide enough to fill the GPU: two M tiles
+    assert E.tile_shape(320, 960, 3, 8, 96, 96) == (64, 2)
+    assert E.tile_shape(640, 640, 3, 8, 48, 48) == (128, 1)
+    # batch 8, 12 x 12 level, 2560 -> 1280: stays at the widest N tile (narrower tiles would move more bytes through L2)
+    assert E.tile_shape(1280, 2560, 3, 8, 12, 12) == (128, 1)
+    # batch 1, same level: 10 of 132 SMs busy with BN = 128 -> narrow N tiles
     assert E.tile_shape(1280, 2560, 3, 1, 12, 12) == (64, 1)
     assert E.tile_shape(1280, 1280, 1, 1, 12, 12, tokens_mode=True)[0] == 64
     # layers the model never touches: Cout < 128 or not a multiple of 64

@@ -102,24 +102,17 @@ def test_cross_attention_two_token_closed_form(synth_state, text_embed):
     torch.testing.assert_close(out, ref, atol=2e-5, rtol=1e-4)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="needs the reference tree (build container only)")
 def test_upsample2d_matches_the_reference_vendored_class():
-    """/root/reference/genpercept/models/dpt_head.py:92-210 vendors diffusers' ``Upsample2D`` — the one block of the
+    """genpercept/models/dpt_head.py:92-210 of the reference vendors diffusers' ``Upsample2D`` — the one block of the
     UNet / VAE graphs whose source IS in the reference tree.  oracle.blocks.Upsample2D (used by every up block of both
-    graphs) must match it, including the explicit-size path diffusers takes when a level has an odd extent."""
-    import importlib.util
-    import sys
-    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-    import make_golden                      # installs the 2-symbol diffusers shim
-    make_golden.load_reference_dpt()
-    ref_mod = sys.modules["ref_dpt_head"]
+    graphs) must match it, including the explicit-size path diffusers takes when a level has an odd extent.  The
+    reference's weights, input and outputs are stored by tests/golden/make_golden_reference.py."""
     from oracle.blocks import Upsample2D
-    torch.manual_seed(3)
-    ref = ref_mod.Upsample2D(24, use_conv=True).eval()
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pipeline.npz"))
     mine = Upsample2D(24).eval()
-    mine.conv.load_state_dict(ref.conv.state_dict())
-    x = torch.randn(2, 24, 7, 9)
+    mine.conv.load_state_dict({"weight": torch.from_numpy(z["up_weight"]), "bias": torch.from_numpy(z["up_bias"])})
+    x = torch.from_numpy(z["up_x"])
     with torch.no_grad():
-        assert torch.equal(mine(x), ref(x))
+        assert torch.equal(mine(x), torch.from_numpy(z["up_out"]))
         for size in ((13, 17), (14, 18), (13, 18)):
-            assert torch.equal(mine(x, size), ref(x, output_size=size))
+            assert torch.equal(mine(x, size), torch.from_numpy(z[f"up_out_{size[0]}x{size[1]}"]))
