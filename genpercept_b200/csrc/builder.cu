@@ -256,10 +256,14 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   static const int stats_mode = std::getenv("GP_STATS") ? std::atoi(std::getenv("GP_STATS")) : 1;
   const bool patch_eligible = gn_fused || (staged && a.mode == 0 && a.ks == 3 && a.srcs.size() == 1 && a.sc.empty() &&
                                            work_px >= 128LL * num_sms && (W % 128) == 0 && !split_ && std::getenv("GP_NO_PATCH") == nullptr);
-  // the patch-resident kernel takes one image row per tile and N tiles of 64: two 50 KiB halo patches, the weight ring and the
-  // 32 KiB accumulator tile fit in shared memory with the statistics scratch of any Cout <= 512
+  // The patch-resident kernel takes one image row per tile (two 50 KiB halo patches).  It keeps a planned N tile of 128 with
+  // the staged epilogue, handing the accumulators over in two 64-column halves through a 32 KiB tile, so at least three
+  // 16 KiB weight stages fit with the statistics scratch of any Cout <= 512; every other plan runs at N = 64.
+  // GP_PATCH_BN=64 (read at plan time): N = 64 everywhere (A/B switch).
   if (patch_eligible) {
-    bn_pre = 64;
+    const char* pbn = std::getenv("GP_PATCH_BN");
+    const bool n128 = bn_pre == 128 && mt_pre == 1 && staged && !(pbn && std::atoi(pbn) == 64);
+    bn_pre = n128 ? 128 : 64;
     mt_pre = 1;
   }
   bool emit_stats = a.want_stats && staged && !is_geglu && Cout <= 512 && stats_mode != 0 && !(stats_mode == 2 && patch_eligible) && !split_;

@@ -20,6 +20,9 @@ namespace gp {
 namespace {
 
 // K loop of the tap-streaming kernel for one (BN, MB = 2 * MT) instance; the whole consumer warpgroup runs it.
+// One batch (the wgmmas of one K block) stays in flight: batch kb is committed before batch kb - 1 is waited for, and
+// batch kb - 1's stage is released only then.  The ring holds >= 2 stages (igemm_finalize), so the stage kb waits for is
+// never the one still held.  Batches into one accumulator run in issue order: the summation order is unchanged.
 template <bool BF16, int BN, int MB>
 __device__ __forceinline__ void tap_consumer(const IgemmParams& p, uint8_t* smem, int stage_bytes, int a_bytes, float* accs,
                                              uint64_t* full_bar, uint64_t* empty_bar, uint64_t* tfull_bar, uint64_t* tempty_bar,
@@ -31,6 +34,7 @@ __device__ __forceinline__ void tap_consumer(const IgemmParams& p, uint8_t* smem
     const TileCoord t = decode_tile(p, tile);
     const int cls = p.cls_from_z0 ? t.z0 : 0;
     const int nkb = p.nkb[cls] * p.npass;
+    int held = -1;                                  // stage read by the batch still in flight
     for (int kb = 0; kb < nkb; ++kb) {
       mbar_wait(&full_bar[stage], phase, 3);
       const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
@@ -46,13 +50,21 @@ __device__ __forceinline__ void tap_consumer(const IgemmParams& p, uint8_t* smem
           wgmma_ss<BN, BF16>(d[mb], a_desc + 2 * k, b_desc + 2 * k, (kb | k) ? 1u : 0u);
       }
       wgmma_commit();
-      wgmma_wait<0>();
+      wgmma_wait<1>();                              // batch kb - 1 has retired
 #pragma unroll
       for (int mb = 0; mb < MB; ++mb) reg_fence(d[mb]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (held >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[held]);
+      }
+      held = stage;
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
     }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int mb = 0; mb < MB; ++mb) reg_fence(d[mb]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[held]);
     mbar_wait(tempty_bar, acc_phase ^ 1, 2);     // the epilogue has read the previous tile
     acc_store<BN, MB>(accs, p.acc_pitch, d, wc, lane);
     mbar_arrive(tfull_bar);
@@ -108,6 +120,23 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_kernel(const __grid_con
   __syncthreads();
   pdl_trigger();      // the next kernel of the stream may be scheduled (it blocks in its own pdl_wait until this grid is done)
   pdl_wait();         // barriers are set up; from here on the predecessor's outputs are read
+
+  // The producer warpgroup gives registers to the other two (igemm_common.cuh).  Each warpgroup's roles sit in their own
+  // branch after its setmaxnreg (ptxas ignores a setmaxnreg from which code of a larger budget is reachable); warps 9 and
+  // 10 take part in the decrease and exit.
+  if (warp < 8) {
+    setmaxnreg_inc<kWorkerRegs>();
+    if (warp >= kConsumerWarp0) {
+      // ===================================================================== wgmma consumer
+      run_tap_consumer<BF16>(p, smem, stage_bytes, a_bytes, accs, full_bar, empty_bar, tfull_bar, tempty_bar, warp - kConsumerWarp0, lane);
+    } else {
+      // ===================================================================== epilogue
+      if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+      else run_epilogue_direct<BF16, kEpiWarps>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
+    }
+    return;
+  }
+  setmaxnreg_dec<kProducerRegs>();
 
   // Single-thread roles run warp-uniform (every lane walks the loop and waits on the barriers) and one
   // elected lane issues: the TMA coordinates then stay in uniform registers.
@@ -168,12 +197,6 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_kernel(const __grid_con
         }
       }
     }
-  } else if (warp >= kConsumerWarp0 && warp < kConsumerWarp0 + 4) {
-    // ===================================================================== wgmma consumer
-    run_tap_consumer<BF16>(p, smem, stage_bytes, a_bytes, accs, full_bar, empty_bar, tfull_bar, tempty_bar, warp - kConsumerWarp0, lane);
-  } else if (warp < kEpiWarps) {
-    if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-    else run_epilogue_direct<BF16, kEpiWarps>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
   }
 }
 
@@ -273,9 +296,14 @@ const char* igemm_finalize(IgemmParams* p) {
   if (p->tma_store && (p->flags & IG_GEGLU) && ((p->Cout % 128) || (p->BN % 128))) return "staged GEGLU needs Cout, BN % 128 == 0";
   if (p->stats && (!p->tma_store || p->Cout > 512 || (p->flags & IG_GEGLU))) return "statistics need the staged epilogue and Cout <= 512";
   p->epi_warps = kEpiWarps;
-  p->acc_pitch = (p->BN + 31) & ~31;
-  // fixed part: staging (one 4 KiB tile per epilogue warp, x2 for the (hi, lo) layout), the accumulator tile, 3 KiB for
-  // barriers and one N tile of bias, the statistics scratch
+  // The patch kernel at BN = 128 hands its tile over in two 64-column halves (igemm_common.cuh): a whole 128 x 128 fp32 tile
+  // (64 KiB) next to the two halo patches would leave room for two weight stages only.
+  p->acc_half = (p->patch && p->BN == 128) ? 1 : 0;
+  if (p->acc_half && (!p->tma_store || p->MT != 1 || (p->flags & IG_GEGLU)))
+    return "patch mode at BN = 128 needs the staged epilogue and MT = 1";
+  p->acc_pitch = p->acc_half ? 64 : (p->BN + 31) & ~31;
+  // fixed part: staging (one 4 KiB tile per epilogue warp, x2 for the (hi, lo) layout), the accumulator tile (or half-tile),
+  // 3 KiB for barriers and one N tile of bias, the statistics scratch
   const int fixed = (p->tma_store ? kEpiWarps * 4096 * (p->out_lo ? 2 : 1) : 0) + acc_tile_bytes(*p) + 3072 + stats_bytes;
   const int ring_unit = p->patch ? p->BN * 128 : kABytes * p->MT + p->BN * 128;   // bytes per pipeline stage
   if (p->patch) {

@@ -9,7 +9,8 @@
 // start coordinate carries the filter-tap offset (halo/padding = TMA out-of-bounds zero fill).
 // B operand: K-major [rows, K] matrix (packed weights, or activations for attention), 3-D map.
 // Accumulators: fp32 in the consumer warpgroup's registers during the K loop, then handed to the epilogue warps
-// through an fp32 tile in shared memory, so the epilogue of tile i overlaps the main loop of tile i+1.
+// through an fp32 tile in shared memory (whole, or in two 64-column halves: acc_half), so the epilogue of tile i
+// overlaps the main loop of tile i+1.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -96,7 +97,9 @@ struct IgemmParams {
                                  // layer has several N tiles and Cout is small enough, all of them (loaded once: bias_all)
   int bias_all;
   int epi_warps;                 // epilogue warps (4: warps 0..3)
-  int acc_pitch;                 // floats per row of the shared accumulator tile (BN rounded up to 32)
+  int acc_pitch;                 // floats per row of the shared accumulator tile (BN rounded up to 32; 64 with acc_half)
+  int acc_half;                  // set by igemm_finalize for the patch kernel at BN = 128: the tile is handed to the epilogue
+                                 // in two 64-column halves through a 64-column shared tile (staged epilogue only)
   int res_prefetch;              // L2-prefetch the next tile's residual boxes one tile period ahead (GP_NO_RES_PREFETCH=1: off)
   CUtensorMap tmRes[kMaxClasses];
   // Patch-resident main loop (igemm_patch.cu; 3x3 stride-1, one source, TW = 128, TH = MT = 1 or 2): per

@@ -5,6 +5,16 @@
 // (its fp32 accumulators live in registers during the K loop), warps 8..11 TMA producers.  At the end of a tile the
 // consumer writes its accumulators into an fp32 tile in shared memory and starts the next tile's K loop while the
 // epilogue warps read that tile one row per thread (tfull / tempty: single buffer, the registers are the second one).
+// Patch-resident tiles at BN = 128 (p.acc_half) hand over in two 64-column halves through a 64-column shared tile: the
+// consumer stores columns 0..63 and arrives tfull, waits tempty, stores columns 64..127 and arrives tfull again; the
+// epilogue reads each half into registers and arrives tempty before it works on it.
+//
+// The consumer's K loop keeps one wgmma batch in flight: it commits batch k, waits until at most one batch is pending
+// (batch k-1 retired) and only then releases the shared-memory stage that batch k-1 read.
+//
+// Registers: the producer warpgroup (warps 8..11, TMA issue only) drops to kProducerRegs per thread at its start and the
+// epilogue and consumer warpgroups rise to kWorkerRegs (128 x 40 + 256 x 232 <= 64 K registers per SM), so the 128
+// accumulators, the transform of the GroupNorm-fused patch kernel and the epilogue's 32-wide vectors fit without spilling.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -20,6 +30,9 @@ constexpr int kMaxSmem = 227 * 1024;
 constexpr int kEpiWarps = 4;                 // warps 0..3
 constexpr int kConsumerWarp0 = 4;            // warps 4..7: the wgmma warpgroup
 constexpr int kRoleThreads = 384;
+constexpr int kProducerRegs = 40;            // setmaxnreg: warps 8..11
+constexpr int kWorkerRegs = 232;             // setmaxnreg: warps 0..7
+static_assert(128 * kProducerRegs + 256 * kWorkerRegs <= 65536, "register file of one SM");
 
 struct TileCoord {
   int n_tile, tx, ty, z0, z1;
@@ -112,16 +125,18 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[BN / 2], uint64_t a, uint64_
 }
 
 // The consumer's register accumulators (MB m64 blocks: tile rows 64 mb ..) -> the shared tile.  wc: warp in the warpgroup.
-template <int BN, int MB>
+// Columns 8 J0 .. 8 (J0 + NJ) - 1 of the accumulators land at tile columns 0 .. 8 NJ - 1 (a half-tile hand-off: J0 = 0 or 8,
+// NJ = 8).
+template <int BN, int MB, int J0 = 0, int NJ = BN / 8>
 __device__ __forceinline__ void acc_store(float* accs, int pitch, float (&d)[MB][BN / 2], int wc, int lane) {
 #pragma unroll
   for (int mb = 0; mb < MB; ++mb) {
     reg_fence(d[mb]);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
+    for (int j = J0; j < J0 + NJ; ++j)
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        const int row = 64 * mb + 16 * wc + (lane >> 2) + 8 * hh, col = 8 * j + 2 * (lane & 3);
+        const int row = 64 * mb + 16 * wc + (lane >> 2) + 8 * hh, col = 8 * (j - J0) + 2 * (lane & 3);
         *reinterpret_cast<float2*>(accs + (size_t)row * pitch + (acc_chunk(col >> 2, row) << 2) + (col & 3)) =
             make_float2(d[mb][4 * j + 2 * hh], d[mb][4 * j + 2 * hh + 1]);
       }
@@ -208,6 +223,9 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
   const bool relu = (p.flags & IG_RELU) != 0;
   constexpr bool geglu = GEGLU;
   const bool do_stats = p.stats != nullptr;
+  // half-tile hand-off (patch kernel, BN = 128, MT = 1, NW = 4: every thread takes every 64-channel group): each group is
+  // one hand-off of the consumer, the shared tile holds that group only
+  const bool halves = !GEGLU && p.acc_half != 0;
   const int etid = threadIdx.x;
   int cur_img = -1;
   int cur_nt = -1;
@@ -230,7 +248,7 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
     const TileCoord t = decode_tile(p, tile);
     const int cls = p.cls_from_z0 ? t.z0 : 0;
     const int n_base = t.n_tile * p.BN;
-    bool waited = false;
+    bool waited = false;   // whole-tile hand-off: tfull of this tile has been waited for
     if (t.n_tile != cur_nt && !p.bias_all) {
       load_bias_tile<NW>(p, sbias, n_base, etid);
       cur_nt = t.n_tile;
@@ -267,7 +285,13 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
       const int sx = t.tx * p.TW + (r0 & (p.TW - 1)), sy = t.ty * p.TH + (r0 >> p.tw_shift);   // store box origin
       for (int c0 = 0; c0 < p.BN; c0 += 64) {
         const int n0 = n_base + c0;
-        if (n0 >= p.Cout) break;
+        if (n0 >= p.Cout) {
+          if (!halves) break;
+          mbar_wait(tfull_bar, acc_phase, 4);     // a half beyond Cout is handed over all the same
+          mbar_arrive(tempty_bar);
+          acc_phase ^= 1;
+          continue;
+        }
         if (!mine(c0)) continue;
         if constexpr (geglu) {   // 128 GEMM columns = 4 x [16 values | 16 gates] -> 64 outputs = one staged 128-byte row
           if (c0 & 64) continue;
@@ -325,6 +349,7 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
           __syncwarp();                                       // every row is in registers before the tile is overwritten
         }
         float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+        uint32_t rh[2][32];                                   // this row's accumulators of the two 32-column pieces
 #pragma unroll
         for (int sub = 0; sub < 2; ++sub) {
           const int ns = n0 + sub * 32;
@@ -346,12 +371,22 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
 #pragma unroll
             for (int q = 0; q < 4; ++q) r2[q] = rp[q];
           }
-          if (!waited) {
-            mbar_wait(tfull_bar, acc_phase, 4);
-            waited = true;
+          if (halves) {
+            if (sub == 0) {      // the whole half into registers: the consumer may store the next one while this one is worked on
+              mbar_wait(tfull_bar, acc_phase, 4);
+              acc_ld<32>(accs, p.acc_pitch, row, 0, rh[0]);
+              acc_ld<32>(accs, p.acc_pitch, row, 32, rh[1]);
+              mbar_arrive(tempty_bar);
+              acc_phase ^= 1;
+            }
+          } else {
+            if (!waited) {
+              mbar_wait(tfull_bar, acc_phase, 4);
+              waited = true;
+            }
+            acc_ld<32>(accs, p.acc_pitch, row, c0 + sub * 32, rh[sub]);
           }
-          uint32_t r[32];
-          acc_ld<32>(accs, p.acc_pitch, row, c0 + sub * 32, r);
+          const uint32_t (&r)[32] = rh[sub];
           float v[32];
 #pragma unroll
           for (int q = 0; q < 32; ++q) v[q] = __uint_as_float(r[q]) + bz[q];
@@ -425,11 +460,13 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
         }   // !GEGLU
       }
     }
-    if (!waited) {
-      mbar_wait(tfull_bar, acc_phase, 4);
+    if (!halves) {
+      if (!waited) {
+        mbar_wait(tfull_bar, acc_phase, 4);
+      }
+      mbar_arrive(tempty_bar);
+      acc_phase ^= 1;
     }
-    mbar_arrive(tempty_bar);
-    acc_phase ^= 1;
   }
   if (lane == 0) tma_store_wait_read0();
   if (do_stats && cur_img >= 0) flush_stats(cur_img);

@@ -108,6 +108,14 @@ __device__ __forceinline__ void transform_patch(const IgemmParams& p, uint32_t s
 }
 
 // K loop of the patch kernel for one (BN, MB = 2 * MT) instance; the whole consumer warpgroup runs it.
+// One batch (the wgmmas of one (chunk, tap)) stays in flight, as in the tap kernel: after batch i is committed and batch
+// i - 1 has retired, batch i - 1's weight stage is released, and so is its patch slot when it was the last batch of its
+// chunk.  The weight ring holds >= 2 stages and there are two patch slots, so nothing waited for is still held.
+// With XFORM, chunk kc + 1's patch is transformed while chunk kc's last batch is in flight: the two read and write
+// different slots, and the slot being transformed was last read by chunk kc - 1, whose batches have all retired (its slot
+// was released only after that, and the producer refilled it only after the release).  The transform's
+// fence.proxy.async + bar.sync 2 still order its stores before the first wgmma that reads them.
+// BN = 128: the tile goes to the epilogue in two 64-column halves (acc_half, igemm_common.cuh).
 template <bool BF16, bool XFORM, int BN, int MB>
 __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* smem, uint8_t* sB, float* accs, uint64_t* a_full,
                                                uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty, uint64_t* tfull_bar,
@@ -122,6 +130,8 @@ __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* sm
   auto row_off = [&](int mb, int dy, int dx) { return ((dy + 1 + (mb >> 1)) * kPP + dx + 1 + (mb & 1) * 64) * 128; };
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = decode_tile(p, tile);
+    int held_stage = -1;     // weight stage of the batch in flight
+    int held_slot = -1;      // patch slot whose last batch is the one in flight
     for (int kc = 0; kc < kc_all; ++kc) {
       const bool main = kc < p.kc_count;
       const bool trm = p.trace != nullptr && blockIdx.x == 0 && wc == 0 && lane == 0;
@@ -148,22 +158,47 @@ __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* sm
           for (int k = 0; k < kBK / 16; ++k) wgmma_ss<BN, BF16>(d[mb], a_desc + 2 * k, b_desc + 2 * k, (kc | tap | k) ? 1u : 0u);
         }
         wgmma_commit();
-        wgmma_wait<0>();
+        wgmma_wait<1>();                            // the previous batch has retired
 #pragma unroll
         for (int mb = 0; mb < MB; ++mb) reg_fence(d[mb]);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&b_empty[stage]);
+        if (held_stage >= 0) {
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(&b_empty[held_stage]);
+            if (held_slot >= 0) mbar_arrive(&a_empty[held_slot]);
+          }
+          held_slot = -1;
+        }
+        held_stage = stage;
         if (++stage == p.stages) { stage = 0; b_phase ^= 1; }
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&a_empty[slot]);
+      held_slot = slot;
       if (trm && mix < 60) p.trace[mix * 8 + 6] = clock64();
       if (++slot == 2) { slot = 0; a_phase ^= 1; }
     }
-    mbar_wait(tempty_bar, acc_phase ^ 1, 2);     // the epilogue has read the previous tile
-    acc_store<BN, MB>(accs, p.acc_pitch, d, wc, lane);
-    mbar_arrive(tfull_bar);
-    acc_phase ^= 1;
+    wgmma_wait<0>();
+#pragma unroll
+    for (int mb = 0; mb < MB; ++mb) reg_fence(d[mb]);
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(&b_empty[held_stage]);
+      mbar_arrive(&a_empty[held_slot]);
+    }
+    if constexpr (BN == 128) {                   // two 64-column halves through the 64-column shared tile
+      mbar_wait(tempty_bar, acc_phase ^ 1, 2);
+      acc_store<BN, MB, 0, 8>(accs, p.acc_pitch, d, wc, lane);
+      mbar_arrive(tfull_bar);
+      acc_phase ^= 1;
+      mbar_wait(tempty_bar, acc_phase ^ 1, 2);
+      acc_store<BN, MB, 8, 8>(accs, p.acc_pitch, d, wc, lane);
+      mbar_arrive(tfull_bar);
+      acc_phase ^= 1;
+    } else {
+      mbar_wait(tempty_bar, acc_phase ^ 1, 2);   // the epilogue has read the previous tile
+      acc_store<BN, MB>(accs, p.acc_pitch, d, wc, lane);
+      mbar_arrive(tfull_bar);
+      acc_phase ^= 1;
+    }
   }
 }
 
@@ -210,21 +245,30 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_patch_kernel(const __gr
   pdl_trigger();      // see ptx.cuh: the next kernel may be scheduled; it blocks in its own pdl_wait
   pdl_wait();         // set-up done; the predecessor grid has completed before any of its outputs is read
 
-  if (warp < kEpiWarps) {
-    // ===================================================================== epilogue
-    if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, true>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-    else epilogue_direct<BF16, kEpiWarps, false>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
-  } else if (warp < kConsumerWarp0 + 4) {
-    // ===================================================================== wgmma consumer
-    const int wc = warp - kConsumerWarp0;
-#define GP_PATCH(BN_, MB_) patch_consumer<BF16, XFORM, BN_, MB_>(p, smem, sB, accs, a_full, a_empty, b_full, b_empty, tfull_bar, tempty_bar, wc, lane)
-    if (p.MT == 2) {
-      if (p.BN == 16) GP_PATCH(16, 4); else if (p.BN == 32) GP_PATCH(32, 4); else GP_PATCH(64, 4);
+  // The producer warpgroup gives registers to the other two (igemm_common.cuh).  Each warpgroup's roles sit in their own
+  // branch after its setmaxnreg (ptxas ignores a setmaxnreg from which code of a larger budget is reachable); warps 9 and
+  // 10 take part in the decrease and exit.
+  if (warp < 8) {
+    setmaxnreg_inc<kWorkerRegs>();
+    if (warp < kEpiWarps) {
+      // ===================================================================== epilogue
+      if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, true>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+      else epilogue_direct<BF16, kEpiWarps, false>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
     } else {
-      if (p.BN == 16) GP_PATCH(16, 2); else if (p.BN == 32) GP_PATCH(32, 2); else if (p.BN == 64) GP_PATCH(64, 2); else GP_PATCH(128, 2);
-    }
+      // ===================================================================== wgmma consumer
+      const int wc = warp - kConsumerWarp0;
+#define GP_PATCH(BN_, MB_) patch_consumer<BF16, XFORM, BN_, MB_>(p, smem, sB, accs, a_full, a_empty, b_full, b_empty, tfull_bar, tempty_bar, wc, lane)
+      if (p.MT == 2) {
+        if (p.BN == 16) GP_PATCH(16, 4); else if (p.BN == 32) GP_PATCH(32, 4); else GP_PATCH(64, 4);
+      } else {
+        if (p.BN == 16) GP_PATCH(16, 2); else if (p.BN == 32) GP_PATCH(32, 2); else if (p.BN == 64) GP_PATCH(64, 2); else GP_PATCH(128, 2);
+      }
 #undef GP_PATCH
-  } else if (warp == 8) {
+    }
+    return;
+  }
+  setmaxnreg_dec<kProducerRegs>();
+  if (warp == 8) {
     // ===================================================================== patch producer
     const bool leader = elect_one();
     int slot = 0;
