@@ -15,10 +15,6 @@ namespace gp {
 size_t Arena::alloc(size_t bytes) {
   bytes = (bytes + 1023) & ~size_t(1023);
   if (bytes == 0) bytes = 1024;
-  // Experiment (GP_ARENA_SKEW=<KiB>): the big VAE tensors are exact multiples of 2^27 bytes, so the input, residual and
-  // output streams of one convolution can sit a power of two apart; a per-allocation skew de-aligns them.
-  static const size_t skew = std::getenv("GP_ARENA_SKEW") ? (size_t)std::atoi(std::getenv("GP_ARENA_SKEW")) * 1024 : 0;
-  if (skew && bytes >= (size_t(1) << 24)) bytes += skew * (1 + (nalloc_++ % 7));
   for (size_t i = 0; i < blks_.size(); ++i) {
     if (blks_[i].free && blks_[i].size >= bytes) {
       if (blks_[i].size > bytes) {
@@ -131,12 +127,11 @@ static void choose_tile(int gw, int gh, int rows, int* tw, int* th, int* shift) 
 // 1).  Two bounds per candidate: the tensor time of the longest-running SM — ceil(tiles / SMs) waves of tiles whose
 // duration scales with the MMA width (a narrow MMA is bound by its operand fetch) — and the L2 -> SM operand traffic,
 // tiles x K x (128 MT + BN) x 2 bytes.  A candidate replaces the default only for a predicted gain above 10 %, so every
-// layer with many waves stays where choose_bn put it.  GP_TILE_MODEL=0: off (A/B switch).
+// layer with many waves stays where choose_bn put it.
 struct TileShape { int bn, mt; };
 template <class MTilesFn>
 static TileShape choose_tile_shape(int cout, double k_elems, int num_sms, TileShape dflt, MTilesFn mtiles_of) {
-  static const bool off = [] { const char* e = std::getenv("GP_TILE_MODEL"); return e && e[0] == '0'; }();
-  if (off || cout % 64 != 0 || cout < 128) return dflt;
+  if (cout % 64 != 0 || cout < 128) return dflt;
   auto cost = [&](TileShape t) {
     const double tiles = (double)mtiles_of(t.mt) * ceil_div(cout, t.bn);
     const double waves = std::ceil(tiles / num_sms);
@@ -184,11 +179,12 @@ static void finalize_or_throw(IgemmParams* p, const std::string& name) {
 
 // The patch-resident kernel with the GroupNorm transform in its operand path (igemm_patch.cu) takes a convolution when:
 // 3x3 stride 1, ONE normalised source (channels % 64 == 0), at most one raw shortcut source, W % 128 == 0, and either the
-// staged epilogue (Cout % 64 == 0) or an fp32 map as output.  Opt-in (GP_GN_FUSE=1): it removes the GroupNorm passes over
-// the big maps, but the transform runs inside the consumer warpgroup, between its wgmma batches.
+// staged epilogue (Cout % 64 == 0) or an fp32 map as output.  Opt-in (GP_GN_FUSE=1) until it has been timed against the
+// unfused path on H100: it removes the GroupNorm passes over the big maps, but the transform runs inside the consumer
+// warpgroup, between its wgmma batches.
 static bool gn_fusable(const ConvArgs& a, bool split) {
   const char* on = std::getenv("GP_GN_FUSE");        // read at plan time (tests toggle it)
-  const bool off = on == nullptr || on[0] == '0' || std::getenv("GP_NO_PATCH") != nullptr;
+  const bool off = on == nullptr || on[0] == '0';
   if (off || split || a.mode != 0 || a.ks != 3 || a.srcs.size() != 1 || a.sc.size() > 1) return false;
   const T4& s = a.srcs[0];
   if ((s.W % 128) || (s.C % 64) || (!a.sc.empty() && (a.sc[0].C % 64))) return false;
@@ -246,27 +242,18 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
     tile_shape_for(Cout, k_elems, tokens_mode, N * (a.mode == 3 ? 4 : 1), (a.mode == 3) ? W : Wo, (a.mode == 3) ? H : Ho, num_sms,
                    &bn_pre, &mt_pre);
   }
-  const bool is_geglu = (a.flags & IG_GEGLU) != 0;
-  const bool staged = !a.out_f32 && std::getenv("GP_DIRECT_EPILOGUE") == nullptr &&
-                      (is_geglu ? (std::getenv("GP_STAGED_GEGLU") != nullptr && !split_ &&   // opt-in: the direct GEGLU stores are the default
-                                   Cout == 2 * a.out.C && (Cout % 128) == 0 && (bn_pre % 128) == 0)
-                                : (Cout == a.out.C && (Cout % 64) == 0 && (bn_pre % 64) == 0));
-  // GP_STATS: 0 = never fuse the GroupNorm partial sums into conv epilogues, 1 = always (default), 2 = everywhere
-  // except the patch-resident layers (whose main loop runs at the tensor-pipe limit, so the epilogue is critical)
-  static const int stats_mode = std::getenv("GP_STATS") ? std::atoi(std::getenv("GP_STATS")) : 1;
+  // the staged (TMA store) epilogue wherever the output allows it; GEGLU and fp32 maps take the direct epilogue
+  const bool staged = !a.out_f32 && !(a.flags & IG_GEGLU) && Cout == a.out.C && (Cout % 64) == 0 && (bn_pre % 64) == 0;
   const bool patch_eligible = gn_fused || (staged && a.mode == 0 && a.ks == 3 && a.srcs.size() == 1 && a.sc.empty() &&
-                                           work_px >= 128LL * num_sms && (W % 128) == 0 && !split_ && std::getenv("GP_NO_PATCH") == nullptr);
+                                           work_px >= 128LL * num_sms && (W % 128) == 0 && !split_);
   // The patch-resident kernel takes one image row per tile (two 50 KiB halo patches).  It keeps a planned N tile of 128 with
   // the staged epilogue, handing the accumulators over in two 64-column halves through a 32 KiB tile, so at least three
   // 16 KiB weight stages fit with the statistics scratch of any Cout <= 512; every other plan runs at N = 64.
-  // GP_PATCH_BN=64 (read at plan time): N = 64 everywhere (A/B switch).
   if (patch_eligible) {
-    const char* pbn = std::getenv("GP_PATCH_BN");
-    const bool n128 = bn_pre == 128 && mt_pre == 1 && staged && !(pbn && std::atoi(pbn) == 64);
-    bn_pre = n128 ? 128 : 64;
+    bn_pre = (bn_pre == 128 && mt_pre == 1 && staged) ? 128 : 64;
     mt_pre = 1;
   }
-  bool emit_stats = a.want_stats && staged && !is_geglu && Cout <= 512 && stats_mode != 0 && !(stats_mode == 2 && patch_eligible) && !split_;
+  bool emit_stats = a.want_stats && staged && Cout <= 512 && !split_;
   if (emit_stats && tokens_mode && ((long long)H * W) % (128 * mt_pre) != 0) emit_stats = false;
   size_t stats_off = 0;
   const size_t stats_bytes = (size_t)N * num_sms * Cout * 2 * sizeof(float);
@@ -424,9 +411,8 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
       }
     }
     // the residual has the output's shape and addressing: same maps over its base
-    if (a.res1 && !a.res2 && !(a.flags & IG_GEGLU) && !split_ && std::getenv("GP_NO_RES_TMA") == nullptr) {
+    if (a.res1 && !a.res2 && !split_) {
       p.res_tma = 1;
-      p.res_prefetch = std::getenv("GP_NO_RES_PREFETCH") == nullptr ? 1 : 0;
       const void* rb = ptr(*a.res1);
       if (tokens) {
         const long long ntok = (long long)N * H * W;
@@ -464,10 +450,7 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
     if (gn_fused) {
       p.gn_ss = gn_ss;
       p.gn_C = s0.C;
-      static const bool tanh32 = std::getenv("GP_PATCH_TANH32") != nullptr;     // A/B switch
-      p.gn_silu = a.gn_silu ? (tanh32 ? 2 : 1) : 0;
-      static const int xmode = std::getenv("GP_PATCH_XFORM") ? std::atoi(std::getenv("GP_PATCH_XFORM")) : 0;
-      p.gn_mode = xmode;
+      p.gn_silu = a.gn_silu ? 1 : 0;
     }
   }
   if (emit_stats) {
@@ -511,14 +494,13 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
   const int C = heads * d;
   const int PL = split_ ? 2 : 1;
   const long long TpP = (long long)Tp * PL;   // physical row pitch of S and V^T
-  static const bool unfused = std::getenv("GP_UNFUSED_ATTN") != nullptr;
   auto set_passes = [&](IgemmParams& p) {
     if (!split_) return;
     p.npass = 3;
     p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
     p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = 1;
   };
-  if (d == 64 && !unfused && !split_) {   // fused wgmma flash-attention kernel (S and P stay on chip)
+  if (d == 64 && !split_) {   // fused wgmma flash-attention kernel (S and P stay on chip)
     if (measuring_) return;
     FattnParams p;
     std::memset(&p, 0, sizeof(p));
@@ -528,7 +510,6 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
     p.T = T; p.heads = heads; p.B = B; p.q_tiles = ceil_div(T, 128);
     p.scale_log2e = 1.4426950408889634f;
     p.bf16 = bf16_ ? 1 : 0;
-    p.trace = fattn_get_trace();
     check_cuda(make_tmap_b(&p.tmQ, q, C, T, B, cs, (long long)T * cs, 128, bf16_), name + ": tmap Q");
     check_cuda(make_tmap_b(&p.tmK, k, C, T, B, cs, (long long)T * cs, 128, bf16_), name + ": tmap K");
     check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, Tp, (long long)C * Tp, 64, bf16_), name + ": tmap Vt");
@@ -810,16 +791,6 @@ void Builder::xattn(const std::string& name, const T4& x, const XattnW& w, float
   push(name, 1, 4.0 * tokens * (double)w.C * w.heads, 2.0 * x.bytes(), [=](cudaStream_t s) {
     return xattn2(xi, yo, tokens, ww.C, ww.heads, ww.U, ww.u0, ww.M, ww.c0, eps, bf, s, sp);
   });
-}
-
-void Builder::geglu_op(const std::string& name, const T4& in, const T4& out) {
-  if (measuring_) return;
-  const void* xi = ptr(in);
-  void* yo = ptr(out);
-  const long long tokens = in.pixels();
-  const int c4 = out.C;
-  const bool bf = bf16_;
-  push(name, 1, 0, (double)in.bytes() + out.bytes(), [=](cudaStream_t s) { return geglu(xi, yo, tokens, c4, bf, s); });
 }
 
 void Builder::relu_op(const std::string& name, const T4& in, const T4& out) {

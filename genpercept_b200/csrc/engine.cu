@@ -18,7 +18,6 @@
 #include <tuple>
 
 #include "engine.h"
-#include "fattn.h"
 
 using namespace gp;
 
@@ -453,15 +452,9 @@ struct gp_engine {
   }
 
   // ------------------------------------------------------------------ graph pieces
-  // 3x3 conv whose input is an NHWC8 tensor with `cin` (3 or 4) real channels: one 64-wide K chunk
-  // per tap through the tensor-core kernel (the TMA box zero-fills channels >= 8).  GP_DIRECT_SMALL=1
-  // routes it through the SIMT direct kernel instead (bring-up triage only).
+  // 3x3 conv whose input is an NHWC8 tensor with `cin` (4 or 8) real channels: one 64-wide K chunk
+  // per tap through the tensor-core kernel (the TMA box zero-fills channels >= 8).
   void small_cin_conv(Builder& b, const std::string& key, const T4& src8, int cin, const T4& out) {
-    static const bool direct = std::getenv("GP_DIRECT_SMALL") != nullptr;
-    if (direct) {
-      b.direct(key, src8, cin, direct_w(key, cin), out, 0, nullptr, 0);
-      return;
-    }
     ConvArgs c;
     c.srcs = {src8};
     c.w = &conv_w(key, {cin});
@@ -721,7 +714,6 @@ struct gp_engine {
     }
     small_cin_conv(b, u + ".conv_in", lat8, unet_in_ch, x);
     std::vector<T4> skips = {x};
-    int cin = 320;
     for (int i = 0; i < 4; ++i) {
       const int cout = kUnetOut[i];
       for (int j = 0; j < 2; ++j) {
@@ -743,9 +735,7 @@ struct gp_engine {
         x = y;
         skips.push_back(x);
       }
-      cin = cout;
     }
-    (void)cin;
     // mid block; x (the last skip) stays alive for the up path
     T4 m0 = resnet(b, u + ".mid_block.resnets.0", {x}, 1280, 1e-5f, true);
     T4 m1 = transformer(b, u + ".mid_block.attentions.0", m0, 20);
@@ -1026,7 +1016,6 @@ struct gp_engine {
     // persistent buffers first so their offsets are identical in both passes
     const size_t in_off = b.raw_alloc((size_t)B * 3 * H * W * 4);
     const size_t out_off = b.raw_alloc((size_t)B * 3 * (H + 64) * (W + 64) * 4);
-    const size_t sums_off = b.raw_alloc((size_t)B * 2560 * 2 * 4);
     const size_t ss_off = b.raw_alloc((size_t)B * 2560 * 2 * 4);
     const size_t mm_off = b.raw_alloc((size_t)B * 2 * 4);
     T4 rgb8 = b.alloc(B, H, W, 32);      // K-packed 3x3 neighbourhoods (preprocess_rgb_im2col); channels 0..2 = the image
@@ -1037,11 +1026,9 @@ struct gp_engine {
       plan->out_dst = plan->out_f32;
       out_f32 = plan->out_f32;
       b.out_slot = &plan->out_dst;
-      b.gn_sums = reinterpret_cast<float*>(b.raw_ptr(sums_off));
       b.gn_ss = reinterpret_cast<float*>(b.raw_ptr(ss_off));
     }
     unsigned int* mm = b.measuring() ? nullptr : reinterpret_cast<unsigned int*>(b.raw_ptr(mm_off));
-    b.stage = GP_STAGE_PRE;   // the preprocess op itself is issued by gp_infer (input dtype varies)
     b.stage = GP_STAGE_VAE_ENCODE;
     T4 latent = vae_encoder(b, rgb8);
     b.stage = GP_STAGE_UNET;
@@ -1857,26 +1844,12 @@ gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int k
     te.e.dev_allocs.push_back(x);
     te.e.dev_allocs.push_back(y);
     GP_CUDA(cudaMemset(x, 0, (size_t)N * H * W * Cin * 2));
-    // a scratch arena for the epilogue statistics (GP_BENCH_STATS=1); externals are addressed relative to it
-    void* scratch = nullptr;
-    GP_CUDA(cudaMalloc(&scratch, (size_t)N * 160 * Cout * 2 * sizeof(float) + (1 << 20)));
-    te.e.dev_allocs.push_back(scratch);
-    Builder b(te.e.bf16, false, reinterpret_cast<uint8_t*>(scratch));
+    Builder b(te.e.bf16, false, nullptr);
     ConvArgs c;
     c.srcs = {b.external(x, N, H, W, Cin)};
     c.ks = ks; c.mode = mode;
     c.w = (mode == 3) ? &te.e.conv_up_w("t") : &te.e.conv_w("t", {Cin});
     c.out = b.external(y, N, Ho, Wo, Cout);
-    if (std::getenv("GP_BENCH_STATS")) c.want_stats = true;      // epilogue experiments: also emit the GroupNorm partial sums
-    void* res = nullptr;
-    T4 rest;
-    if (std::getenv("GP_BENCH_RES")) {              // ... and / or add a residual of the output's shape
-      GP_CUDA(cudaMalloc(&res, (size_t)N * Ho * Wo * Cout * 2));
-      GP_CUDA(cudaMemset(res, 0, (size_t)N * Ho * Wo * Cout * 2));
-      te.e.dev_allocs.push_back(res);
-      rest = b.external(res, N, Ho, Wo, Cout);
-      c.res1 = &rest;
-    }
     b.conv("bench", c);
     cudaEvent_t e0, e1;
     GP_CUDA(cudaEventCreate(&e0));
@@ -1894,13 +1867,5 @@ gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int k
     if (flops) *flops = b.ops[0].flops;
   });
 }
-
-/* debug: device buffer of >= 512 int64; CTA 0 of subsequent patch-kernel launches stamps clock64() per K chunk i < 60:
-   [i*8+4] consumer starts waiting for the patch, +5 patch ready (transformed if GroupNorm-fused), +6 all taps issued and retired */
-void gp_debug_patch_trace(void* dev_buf) { gp::igemm_patch_set_trace(reinterpret_cast<long long*>(dev_buf)); }
-
-/* debug: device buffer of >= 512 int64 that CTA 0 of subsequently planned fused-attention launches fills with clock64() stamps
-   ([j*8+0] key block j starts, +1 S done, +2 P.V done; j < 64) */
-void gp_debug_fattn_trace(void* dev_buf) { gp::fattn_set_trace(reinterpret_cast<long long*>(dev_buf)); }
 
 }  // extern "C"

@@ -74,7 +74,6 @@ class Arena {
   struct Blk { size_t off, size; bool free; };
   std::vector<Blk> blks_;
   size_t high_ = 0;
-  size_t nalloc_ = 0;
 };
 
 struct Op {
@@ -136,7 +135,6 @@ class Builder {
   void gn_scale_shift(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps);
   void ln(const std::string& name, const T4& x, const NormW& nw, float eps, const T4& out);
   void xattn(const std::string& name, const T4& x, const XattnW& w, float eps, const T4& out);
-  void geglu_op(const std::string& name, const T4& in, const T4& out);
   void relu_op(const std::string& name, const T4& in, const T4& out);
   void bilinear(const std::string& name, const T4& in, const T4& out);
   void direct(const std::string& name, const T4& in, int cin, const DirectW& w, const T4& out, int flags,
@@ -153,7 +151,6 @@ class Builder {
   bool bf16() const { return bf16_; }
   bool measuring() const { return measuring_; }
   size_t arena_bytes() const { return arena_.high_water(); }
-  float* gn_sums = nullptr;   // [N][Cmax][2]
   float* gn_ss = nullptr;
   // When set, ops that write the final fp32 map (ConvArgs::out_f32 / direct(..., out_f32)) read their destination from
   // *out_slot at LAUNCH time, so gp_infer can point them at the caller's device buffer (no copy of the result).

@@ -81,8 +81,6 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();      // see ptx.cuh: the next kernel may be scheduled; it blocks in its own pdl_wait
-  pdl_wait();         // set-up done; the predecessor grid has completed before any of its outputs is read
 
   if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer (whole warp waits, one lane issues)
@@ -107,7 +105,6 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
     const int g = warp >> 2, wc = warp & 3;
     const float c2 = p.scale_log2e;
     const uint64_t q_desc = make_sw128_kmajor_desc(smem_u32(sQ + g * (kQBytes / 2)));
-    const bool tr = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
     float o[32];
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows r and r + 8 of this thread
 #pragma unroll
@@ -115,7 +112,6 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
     mbar_wait(q_full, 0, 12);
     for (int j = 0; j < nblk; ++j) {
       const int st = j % kStages;
-      if (tr && j < 64) p.trace[j * 8 + 0] = clock64();
       mbar_wait(&kv_full[st], (j / kStages) & 1, 11);
       float s[64];
       const uint64_t k_desc = make_sw128_kmajor_desc(smem_u32(sK + st * kKBytes));
@@ -126,7 +122,6 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
       wgmma_commit();
       wgmma_wait<0>();
       reg_fence(s);
-      if (tr && j < 64) p.trace[j * 8 + 1] = clock64();
       // s[4i + e]: key 8i + 2 (lane & 3) + (e & 1), row r (e < 2) or r + 8
       const int kvalid = T - j * 128;
       if (kvalid < 128) {
@@ -179,7 +174,6 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
       reg_fence(o);
       __syncwarp();
       if (lane == 0) mbar_arrive(&kv_empty[st]);
-      if (tr && j < 64) p.trace[j * 8 + 2] = clock64();
     }
     // normalise, store: rows r and r + 8, columns 8 i + 2 (lane & 3) + {0, 1}
     const float inv0 = 1.f / quad_sum(l0), inv1 = 1.f / quad_sum(l1);
@@ -199,10 +193,6 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
 }
 
 }  // namespace
-
-static long long* g_trace = nullptr;
-void fattn_set_trace(long long* dev_buf) { g_trace = dev_buf; }
-long long* fattn_get_trace() { return g_trace; }
 
 cudaError_t fattn_launch(const FattnParams& p, cudaStream_t stream) {
   static bool attr_dev[64] = {};

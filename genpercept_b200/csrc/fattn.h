@@ -15,11 +15,7 @@ struct FattnParams {
   int T, heads, B, q_tiles;
   float scale_log2e;
   int bf16;
-  long long* trace;   // debug: CTA 0 records clock64() per key block (start, S done, P.V done; null = off)
 };
-
-void fattn_set_trace(long long* dev_buf);   // applies to subsequently built FattnParams (debug only)
-long long* fattn_get_trace();
 
 cudaError_t fattn_launch(const FattnParams& p, cudaStream_t stream);
 

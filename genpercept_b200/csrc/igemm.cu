@@ -9,7 +9,6 @@
 // accumulators in registers, at most 128 per thread.
 #include "igemm.h"
 
-#include <cstdlib>
 #include <cstring>
 
 #include "igemm_common.cuh"
@@ -118,8 +117,6 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_kernel(const __grid_con
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();      // the next kernel of the stream may be scheduled (it blocks in its own pdl_wait until this grid is done)
-  pdl_wait();         // barriers are set up; from here on the predecessor's outputs are read
 
   // The producer warpgroup gives registers to the other two (igemm_common.cuh).  Each warpgroup's roles sit in their own
   // branch after its setmaxnreg (ptxas ignores a setmaxnreg from which code of a larger budget is reachable); warps 9 and
@@ -131,8 +128,8 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_kernel(const __grid_con
       run_tap_consumer<BF16>(p, smem, stage_bytes, a_bytes, accs, full_bar, empty_bar, tfull_bar, tempty_bar, warp - kConsumerWarp0, lane);
     } else {
       // ===================================================================== epilogue
-      if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-      else run_epilogue_direct<BF16, kEpiWarps>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
+      if (p.tma_store) run_epilogue_staged<BF16, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+      else run_epilogue_direct<BF16>(p, sbias, tfull_bar, tempty_bar, accs, warp, lane);
     }
     return;
   }
@@ -257,10 +254,6 @@ cudaError_t make_tmap_b(CUtensorMap* m, const void* base, long long K, long long
 
 static int acc_tile_bytes(const IgemmParams& p) { return 128 * p.MT * p.acc_pitch * (int)sizeof(float); }
 
-size_t igemm_smem_bytes(const IgemmParams& p) {
-  return (size_t)p.stages * (kABytes * p.MT + p.BN * 128) + acc_tile_bytes(p) + (2 * p.stages + 6) * 8 + 16 + 1024;
-}
-
 const char* igemm_finalize(IgemmParams* p) {
   if (p->MT == 0) p->MT = 1;
   if (p->npass == 0) p->npass = 1;
@@ -291,15 +284,13 @@ const char* igemm_finalize(IgemmParams* p) {
   if (total > 0x7fffffffLL) return "too many tiles";
   p->total_tiles = (int)total;
   const int stats_bytes = p->stats ? 4 * p->Cout * 2 * (int)sizeof(float) : 0;
-  if (p->tma_store && ((p->Cout % 64) || (p->BN % 64) || (p->flags & IG_OUT_F32_NCHW) || p->out_z0 != 0))
-    return "staged epilogue needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output";
-  if (p->tma_store && (p->flags & IG_GEGLU) && ((p->Cout % 128) || (p->BN % 128))) return "staged GEGLU needs Cout, BN % 128 == 0";
-  if (p->stats && (!p->tma_store || p->Cout > 512 || (p->flags & IG_GEGLU))) return "statistics need the staged epilogue and Cout <= 512";
-  p->epi_warps = kEpiWarps;
+  if (p->tma_store && ((p->Cout % 64) || (p->BN % 64) || (p->flags & (IG_OUT_F32_NCHW | IG_GEGLU)) || p->out_z0 != 0))
+    return "staged epilogue needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output, no GEGLU";
+  if (p->stats && (!p->tma_store || p->Cout > 512)) return "statistics need the staged epilogue and Cout <= 512";
   // The patch kernel at BN = 128 hands its tile over in two 64-column halves (igemm_common.cuh): a whole 128 x 128 fp32 tile
   // (64 KiB) next to the two halo patches would leave room for two weight stages only.
   p->acc_half = (p->patch && p->BN == 128) ? 1 : 0;
-  if (p->acc_half && (!p->tma_store || p->MT != 1 || (p->flags & IG_GEGLU)))
+  if (p->acc_half && (!p->tma_store || p->MT != 1))
     return "patch mode at BN = 128 needs the staged epilogue and MT = 1";
   p->acc_pitch = p->acc_half ? 64 : (p->BN + 31) & ~31;
   // fixed part: staging (one 4 KiB tile per epilogue warp, x2 for the (hi, lo) layout), the accumulator tile (or half-tile),
@@ -319,7 +310,7 @@ const char* igemm_finalize(IgemmParams* p) {
   // loaded once instead of on every change of tile column, unless that costs a pipeline stage
   p->bias_slots = kBiasSlots;
   p->bias_all = 0;
-  if (p->n_tiles_n > 1 && p->n_tiles_n * p->BN + 32 <= 4096 && getenv("GP_NO_BIAS_ALL") == nullptr) {
+  if (p->n_tiles_n > 1 && p->n_tiles_n * p->BN + 32 <= 4096) {
     const int extra = (p->n_tiles_n * p->BN + 32 - kBiasSlots) * (int)sizeof(float);
     if ((avail - extra) / ring_unit == st) {
       p->bias_all = 1;
@@ -330,13 +321,6 @@ const char* igemm_finalize(IgemmParams* p) {
   if (st < 2) return "tile too large for shared memory";
   p->stages = st;
   return nullptr;
-}
-
-static cudaError_t igemm_init();
-
-int igemm_grid(const IgemmParams& p) {
-  if (igemm_init() != cudaSuccess) return 0;
-  return p.total_tiles < g_num_sms ? p.total_tiles : g_num_sms;
 }
 
 // Function attributes are per device: keyed by the current device so that engines on several GPUs of one process work.

@@ -82,11 +82,11 @@ struct IgemmParams {
   //   stats[((image * stats_slots + blockIdx.x) * Cout + c) * 2 + {0, 1}]
   // Pre-zeroed by the caller (CTAs that see no tile of an image do not write its slot).
   float* stats;
-  int stats_slots;               // >= gridDim.x (igemm_grid())
+  int stats_slots;               // >= gridDim.x (min(total_tiles, SM count), igemm_launch)
   int stats_hw;                  // tokens mode (Z1 == 1, gridH == 1): pixels per image; else 0
   // Staged epilogue: each epilogue warp writes its 32 rows x 64 channels (16-bit) into a swizzled
   // shared-memory tile and issues one TMA store (full 128-byte lines, image-edge clipping by the
-  // tensor map).  Needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output.  One map per class.
+  // tensor map).  Needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output, no GEGLU.  One map per class.
   int tma_store;
   CUtensorMap tmOut[kMaxClasses];   // (C, W, H, N) views of the output, box (64, min(TW,32), 32/min(TW,32), 1)
   // Residual through TMA (staged epilogue, res1 only): the same boxes of the residual tensor are LOADED into the
@@ -96,11 +96,9 @@ struct IgemmParams {
   int bias_slots;                // floats of shared memory holding the bias: 288 (one N tile, reloaded per tile) or, when the
                                  // layer has several N tiles and Cout is small enough, all of them (loaded once: bias_all)
   int bias_all;
-  int epi_warps;                 // epilogue warps (4: warps 0..3)
   int acc_pitch;                 // floats per row of the shared accumulator tile (BN rounded up to 32; 64 with acc_half)
   int acc_half;                  // set by igemm_finalize for the patch kernel at BN = 128: the tile is handed to the epilogue
                                  // in two 64-column halves through a 64-column shared tile (staged epilogue only)
-  int res_prefetch;              // L2-prefetch the next tile's residual boxes one tile period ahead (GP_NO_RES_PREFETCH=1: off)
   CUtensorMap tmRes[kMaxClasses];
   // Patch-resident main loop (igemm_patch.cu; 3x3 stride-1, one source, TW = 128, TH = MT = 1 or 2): per
   // 64-channel K chunk ONE (TH+2) x (TW+2) halo patch is loaded and all nine taps are fed from it by
@@ -115,17 +113,12 @@ struct IgemmParams {
   CUtensorMap tmPatch2;          // same box over the shortcut source
   // GroupNorm(+SiLU) of the patch source applied in shared memory before the MMA reads it (patch mode only):
   // y = silu(x * scale + shift), (scale, shift) = gn_ss[(image * gn_C + channel) * 2 + {0, 1}] (gn_finalize's output).
-  long long* trace;              // debug (gp_debug_patch_trace): CTA 0 stamps clock64() at slots 8k+4..8k+6 of K chunk k; null = off
   const float* gn_ss;            // null: the source is used as it is
   int gn_C;                      // channels of the normalised tensor (= the patch source's)
-  int gn_silu;
-  int gn_mode;                   // experiment switches of the transform loop (GP_PATCH_XFORM), see igemm_patch.cu
+  int gn_silu;                   // 1: SiLU after the affine, 0: affine only
 };
 
 cudaError_t igemm_patch_launch(const IgemmParams& p, int grid, cudaStream_t stream);   // igemm_patch.cu
-void igemm_patch_set_trace(long long* dev_buf);   // applies to subsequent launches (debug only)
-
-int igemm_grid(const IgemmParams& p);   // CTAs that igemm_launch will use for p (after igemm_finalize)
 
 // host helpers ----------------------------------------------------------------------------------
 // Encode a 4-D NHWC view (C, W, H, N) with element strides (sW, sH, sN) and box (64, TW, TH, 1).
@@ -137,6 +130,5 @@ cudaError_t make_tmap_b(CUtensorMap* m, const void* base, long long K, long long
 // Fill tile counts / stage count and validate; returns nullptr or an error string.
 const char* igemm_finalize(IgemmParams* p);
 cudaError_t igemm_launch(const IgemmParams& p, cudaStream_t stream);
-size_t igemm_smem_bytes(const IgemmParams& p);
 
 }  // namespace gp

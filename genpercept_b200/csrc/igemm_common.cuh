@@ -161,11 +161,8 @@ __device__ __forceinline__ float gelu_erf(float g) {
   return g * (g >= 0.f ? 1.f - q : q);
 }
 
-// NW epilogue warps (4 or 8).  With 8, warps w and w + 4 read the same accumulator rows (32 * (w % 4) ...) and split the
-// tile's 64-channel groups between them.
-template <int NW>
 __device__ __forceinline__ void epi_sync() {   // the epilogue threads only
-  asm volatile("bar.sync 1, %0;" ::"n"(NW * 32) : "memory");
+  asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32) : "memory");
 }
 
 // The bias of the CTA's current N tile lives in shared memory (kBiasSlots floats, zero beyond Cout): every 32-column piece
@@ -175,15 +172,14 @@ constexpr int kBiasSlots = 288;
 // A layer with several N tiles changes tile column on every tile of a CTA (tiles are numbered N-fastest and taken with a
 // stride of gridDim.x), i.e. two barriers of all epilogue warps plus an L2 round trip per tile: when the padded Cout fits
 // (p.bias_all, igemm_finalize) the whole bias vector is loaded once instead.
-template <int NW>
 __device__ __forceinline__ void load_bias_tile(const IgemmParams& p, float* sbias, int n_base, int etid) {
-  epi_sync<NW>();                              // nobody still reads the previous tile's values
+  epi_sync();                                  // nobody still reads the previous tile's values
   const int count = p.bias_all ? p.bias_slots : kBiasSlots;
-  for (int i = etid; i < count; i += NW * 32) {
+  for (int i = etid; i < count; i += kEpiWarps * 32) {
     const int n = n_base + i;
     sbias[i] = (p.bias != nullptr && n < p.Cout) ? __ldg(p.bias + n) : 0.f;
   }
-  epi_sync<NW>();
+  epi_sync();
 }
 __device__ __forceinline__ void bias32(const float* sbias, int c, float (&bz)[32]) {
 #pragma unroll
@@ -196,9 +192,9 @@ __device__ __forceinline__ void bias32(const float* sbias, int c, float (&bz)[32
 // Staged epilogue (shared by the tap-streaming and the patch-resident main loops): accumulator tile -> registers
 // (bias / residuals / ReLU) -> 16-bit rows in a SWIZZLE_128B shared tile -> one TMA store per
 // (warp, 64-channel group), plus the GroupNorm partial sums read back column-wise from the tile.
-// SPLIT / RES / GEGLU are compile-time: with run-time flags every 32 x 64 piece pays the moves and branches around the
-// variants not taken.  RES: 0 none, 1 residual tile through TMA, 2 per-thread rows.
-template <bool BF16, int NW, bool SPLIT, int RES, bool GEGLU>
+// SPLIT / RES are compile-time: with run-time flags every 32 x 64 piece pays the moves and branches around the variants
+// not taken.  RES: 0 none, 1 residual tile through TMA, 2 per-thread rows.
+template <bool BF16, bool SPLIT, int RES>
 __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* stg_base, float* sacc, float* sbias, uint64_t* tfull_bar,
                                                 uint64_t* tempty_bar, uint64_t* res_bar, const float* accs, int warp, int lane) {
   // ===================================================================== epilogue, staged + TMA store
@@ -206,65 +202,59 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
   // one TMA store per (warp, 64-channel group): full-line writes instead of 16-byte pieces at a
   // 2C-byte stride, and image-edge clipping for free.  GroupNorm partial sums are read back
   // column-wise from the staged tile (conflict-free), in a fixed order.
-  const int wq = warp & 3;                   // epilogue warps are warps 0..NW-1; warp % 4 -> tile rows [32*wq, +32)
-  const int half = warp >> 2;                // NW == 8: which of the tile's 64-channel groups this warp takes (parity)
+  const int wq = warp;                       // tile rows [32*wq, +32)
   uint8_t* stg = stg_base + warp * 4096;
   const uint32_t stg_addr = smem_u32(stg);
   const uint32_t my_row = stg_addr + lane * 128;
-  constexpr bool split = SPLIT;              // high-precision mode: a second staged tile (+NW * 4 KiB) takes the lo plane
-  const uint32_t my_row_lo = my_row + NW * 4096;
-  // 64-channel groups (128 GEMM columns with GEGLU) of the N tile go to the two halves by parity; a tile with one group only
-  // is done by half 0 (statistics: the halves then never accumulate the same channel into sacc[wq])
-  constexpr int gshift = GEGLU ? 7 : 6;
-  const bool two_groups = NW == 8 && (p.BN >> gshift) >= 2;
-  auto mine = [&](int c0) { return NW == 4 || (two_groups ? ((c0 >> gshift) & 1) == half : half == 0); };
+  constexpr bool split = SPLIT;              // high-precision mode: a second staged tile (+kEpiWarps * 4 KiB) takes the lo plane
+  const uint32_t my_row_lo = my_row + kEpiWarps * 4096;
   const int sw = lane & 7;
   uint32_t acc_phase = 0, res_phase = 0;
   const bool relu = (p.flags & IG_RELU) != 0;
-  constexpr bool geglu = GEGLU;
   const bool do_stats = p.stats != nullptr;
-  // half-tile hand-off (patch kernel, BN = 128, MT = 1, NW = 4: every thread takes every 64-channel group): each group is
-  // one hand-off of the consumer, the shared tile holds that group only
-  const bool halves = !GEGLU && p.acc_half != 0;
+  // half-tile hand-off (patch kernel, BN = 128, MT = 1): each 64-channel group is one hand-off of the consumer, the shared
+  // tile holds that group only
+  const bool halves = p.acc_half != 0;
   const int etid = threadIdx.x;
   int cur_img = -1;
   int cur_nt = -1;
+  // sum the four warp-private accumulators in a fixed order, publish this CTA's slot, reset
   auto flush_stats = [&](int img) {
-    epi_sync<NW>();
+    epi_sync();
     float* dst = p.stats + ((long long)img * p.stats_slots + blockIdx.x) * p.Cout * 2;
-    for (int i = etid; i < 2 * p.Cout; i += NW * 32) {
+    for (int i = etid; i < 2 * p.Cout; i += kEpiWarps * 32) {
       const float tot = (sacc[i] + sacc[2 * p.Cout + i]) + (sacc[4 * p.Cout + i] + sacc[6 * p.Cout + i]);
       dst[i] = tot;
       sacc[i] = 0.f; sacc[2 * p.Cout + i] = 0.f; sacc[4 * p.Cout + i] = 0.f; sacc[6 * p.Cout + i] = 0.f;
     }
-    epi_sync<NW>();
+    epi_sync();
   };
   if (do_stats) {
-    for (int i = etid; i < 8 * p.Cout; i += NW * 32) sacc[i] = 0.f;
-    epi_sync<NW>();
+    for (int i = etid; i < 8 * p.Cout; i += kEpiWarps * 32) sacc[i] = 0.f;
+    epi_sync();
   }
-  if (p.bias_all) load_bias_tile<NW>(p, sbias, 0, etid);
+  if (p.bias_all) load_bias_tile(p, sbias, 0, etid);
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = decode_tile(p, tile);
     const int cls = p.cls_from_z0 ? t.z0 : 0;
     const int n_base = t.n_tile * p.BN;
     bool waited = false;   // whole-tile hand-off: tfull of this tile has been waited for
     if (t.n_tile != cur_nt && !p.bias_all) {
-      load_bias_tile<NW>(p, sbias, n_base, etid);
+      load_bias_tile(p, sbias, n_base, etid);
       cur_nt = t.n_tile;
     }
     const int bias_origin = p.bias_all ? 0 : n_base;
     // The residual boxes of this CTA's NEXT tile are pulled into L2 now, a whole tile period before their TMA loads:
     // those loads sit serially in front of every 32 x 64 piece of the epilogue, and at DRAM latency under load four of
     // them per warp can outlast the main loop of the short-K (Cout = 128) layers.
-    if (RES == 1 && p.res_prefetch && lane == 0 && tile + (int)gridDim.x < p.total_tiles) {
+    if (RES == 1 && lane == 0 && tile + (int)gridDim.x < p.total_tiles) {
       const TileCoord tn = decode_tile(p, tile + gridDim.x);
       const int ncls = p.cls_from_z0 ? tn.z0 : 0;
       for (int h = 0; h < p.MT; ++h) {
         const int r0 = h * 128 + wq * 32;
         const int psx = tn.tx * p.TW + (r0 & (p.TW - 1)), psy = tn.ty * p.TH + (r0 >> p.tw_shift);
         for (int c0 = 0; c0 < p.BN && tn.n_tile * p.BN + c0 < p.Cout; c0 += 64)
-          if (mine(c0)) tma_prefetch_l2_4d(&p.tmRes[ncls], tn.n_tile * p.BN + c0, psx, psy, tn.z1);
+          tma_prefetch_l2_4d(&p.tmRes[ncls], tn.n_tile * p.BN + c0, psx, psy, tn.z1);
       }
     }
     if (do_stats) {
@@ -292,46 +282,7 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
           acc_phase ^= 1;
           continue;
         }
-        if (!mine(c0)) continue;
-        if constexpr (geglu) {   // 128 GEMM columns = 4 x [16 values | 16 gates] -> 64 outputs = one staged 128-byte row
-          if (c0 & 64) continue;
-          if (lane == 0) tma_store_wait_read0();
-          __syncwarp();
-#pragma unroll
-          for (int sub = 0; sub < 4; ++sub) {
-            const int ns = n0 + sub * 32;
-            float bz[32];
-            bias32(sbias, ns - bias_origin, bz);
-            if (!waited) {
-              mbar_wait(tfull_bar, acc_phase, 4);
-              waited = true;
-            }
-            uint32_t r[32];
-            acc_ld<32>(accs, p.acc_pitch, row, c0 + sub * 32, r);
-            float g[16];
-#pragma unroll
-            for (int q = 0; q < 16; ++q) {
-              const float a = __uint_as_float(r[q]) + bz[q], gt = __uint_as_float(r[16 + q]) + bz[16 + q];
-              g[q] = valid ? a * gelu_erf(gt) : 0.f;
-            }
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const uint32_t a = my_row + (((sub * 2 + i) ^ sw) << 4);
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(pack16<BF16>(g[8 * i], g[8 * i + 1])),
-                           "r"(pack16<BF16>(g[8 * i + 2], g[8 * i + 3])), "r"(pack16<BF16>(g[8 * i + 4], g[8 * i + 5])),
-                           "r"(pack16<BF16>(g[8 * i + 6], g[8 * i + 7]))
-                           : "memory");
-            }
-          }
-          fence_proxy_async_shared();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_4d(&p.tmOut[cls], stg_addr, n0 >> 1, sx, sy, t.z1);
-            tma_store_commit();
-          }
-          continue;
-        } else {
-        if (lane == 0) tma_store_wait_read0();                // the previous store has finished reading the tile
+        if (lane == 0) tma_store_wait_read0();               // the previous store has finished reading the tile
         __syncwarp();
         uint4 rt[8];                                          // this thread's residual row (64 channels), res_tma only
         if constexpr (RES == 1) {
@@ -440,7 +391,7 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
         __syncwarp();
         if (lane == 0) {
           tma_store_4d(&p.tmOut[cls], stg_addr, n0, sx, sy, t.z1);
-          if (split) tma_store_4d(&p.tmOutLo[cls], stg_addr + NW * 4096, n0, sx, sy, t.z1);
+          if (split) tma_store_4d(&p.tmOutLo[cls], stg_addr + kEpiWarps * 4096, n0, sx, sy, t.z1);
           tma_store_commit();
         }
         if (do_stats) {
@@ -457,7 +408,6 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
           float* d = sacc + ((size_t)wq * p.Cout + n0 + 2 * lane) * 2;
           d[0] += s0; d[1] += q0; d[2] += s1; d[3] += q1;
         }
-        }   // !GEGLU
       }
     }
     if (!halves) {
@@ -473,38 +423,33 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
 }
 
 
-// Run-time flags -> the specialised staged epilogue.  LEAN (the patch-resident kernel): no (hi, lo) layout, no GEGLU.
-template <bool BF16, int NW, bool LEAN>
+// Run-time flags -> the specialised staged epilogue.  LEAN (the patch-resident kernel): no (hi, lo) layout.
+template <bool BF16, bool LEAN>
 __device__ __forceinline__ void run_epilogue_staged(const IgemmParams& p, uint8_t* stg_base, float* sacc, float* sbias, uint64_t* tfull_bar,
                                                     uint64_t* tempty_bar, uint64_t* res_bar, const float* accs, int warp, int lane) {
   const int rm = p.res_tma ? 1 : ((p.res1 != nullptr || p.res2 != nullptr) ? 2 : 0);
   if constexpr (!LEAN) {
-    if (p.flags & IG_GEGLU) {
-      epilogue_staged<BF16, NW, false, 0, true>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-      return;
-    }
     if (p.out_lo != 0) {
-      if (rm == 2) epilogue_staged<BF16, NW, true, 2, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-      else epilogue_staged<BF16, NW, true, 0, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+      if (rm == 2) epilogue_staged<BF16, true, 2>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+      else epilogue_staged<BF16, true, 0>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
       return;
     }
   }
-  if (rm == 1) epilogue_staged<BF16, NW, false, 1, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-  else if (rm == 2) epilogue_staged<BF16, NW, false, 2, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-  else epilogue_staged<BF16, NW, false, 0, false>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+  if (rm == 1) epilogue_staged<BF16, false, 1>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+  else if (rm == 2) epilogue_staged<BF16, false, 2>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+  else epilogue_staged<BF16, false, 0>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
 }
 
 // Direct epilogue: accumulator tile -> registers (bias / residuals / ReLU / affine clamp / GEGLU) -> global stores straight from
-// the registers: fp32 NCHW maps, odd channel counts, GEGLU, the high-precision (hi, lo) layout.
+// the registers: fp32 NCHW maps, odd channel counts, GEGLU, the high-precision (hi, lo) layout.  No GroupNorm statistics:
+// those are produced by the staged (TMA store) epilogue only.
 // LEAN = the GEGLU projection of the default mode (full 32-column chunks, no residual, 16-bit output, no (hi, lo) planes): every
 // other variant is compiled out of its loop (same reasoning as the staged epilogue's template parameters).
-template <bool BF16, int NW, bool LEAN>
-__device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sacc, float* sbias, uint64_t* tfull_bar, uint64_t* tempty_bar,
+template <bool BF16, bool LEAN>
+__device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sbias, uint64_t* tfull_bar, uint64_t* tempty_bar,
                                                 const float* accs, int warp, int lane) {
   // ===================================================================== epilogue
-  const int wq = warp & 3;                 // warp % 4 -> tile rows [32*wq, 32*wq+32)
-  const int half = warp >> 2;              // NW == 8: the tile's 32-column chunks go to the two halves by parity
-  const bool two_chunks = NW == 8 && p.BN > 32;
+  const int wq = warp;                     // tile rows [32*wq, 32*wq+32)
   uint32_t acc_phase = 0;
   const bool f32out = !LEAN && (p.flags & IG_OUT_F32_NCHW) != 0;
   const bool relu = !LEAN && (p.flags & IG_RELU) != 0;
@@ -513,43 +458,19 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sac
   const void* const res1 = LEAN ? nullptr : p.res1;
   const void* const res2 = LEAN ? nullptr : p.res2;
   const long long out_lo = LEAN ? 0 : p.out_lo;
-  const bool do_stats = false;               // statistics are produced by the staged (TMA store) epilogue only
   const int etid = threadIdx.x;              // 0..127 among the epilogue threads
-  int cur_img = -1;
   int cur_nt = -1;
-  // sum the four warp-private accumulators in a fixed order, publish this CTA's slot, reset
-  auto flush_stats = [&](int img) {
-    epi_sync<NW>();
-    float* dst = p.stats + ((long long)img * p.stats_slots + blockIdx.x) * p.Cout * 2;
-    for (int i = etid; i < 2 * p.Cout; i += NW * 32) {
-      const float tot = (sacc[i] + sacc[2 * p.Cout + i]) + (sacc[4 * p.Cout + i] + sacc[6 * p.Cout + i]);
-      dst[i] = tot;
-      sacc[i] = 0.f; sacc[2 * p.Cout + i] = 0.f; sacc[4 * p.Cout + i] = 0.f; sacc[6 * p.Cout + i] = 0.f;
-    }
-    epi_sync<NW>();
-  };
-  if (do_stats) {
-    for (int i = etid; i < 8 * p.Cout; i += NW * 32) sacc[i] = 0.f;
-    epi_sync<NW>();
-  }
-  if (p.bias_all) load_bias_tile<NW>(p, sbias, 0, etid);
+  if (p.bias_all) load_bias_tile(p, sbias, 0, etid);
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = decode_tile(p, tile);
     const int cls = p.cls_from_z0 ? t.z0 : 0;
     const int n_base = t.n_tile * p.BN;
     bool waited = false;
     if (t.n_tile != cur_nt && !p.bias_all) {
-      load_bias_tile<NW>(p, sbias, n_base, etid);
+      load_bias_tile(p, sbias, n_base, etid);
       cur_nt = t.n_tile;
     }
     const int bias_origin = p.bias_all ? 0 : n_base;
-    if (do_stats) {
-      const int img = p.stats_hw ? (t.tx * p.TW) / p.stats_hw : t.z1;
-      if (img != cur_img) {
-        if (cur_img >= 0) flush_stats(cur_img);
-        cur_img = img;
-      }
-    }
     for (int h = 0; h < p.MT; ++h) {
       const int row = h * 128 + wq * 32 + lane;
       const int ti = row >> p.tw_shift, tj = row & (p.TW - 1);
@@ -559,7 +480,6 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sac
       const long long pix_off = t.z1 * p.out_z1 + t.z0 * p.out_z0 + (long long)oy * p.out_row_stride +
                                 (long long)ox * p.out_pix_stride;
       for (int c0 = 0; c0 < p.BN; c0 += 32) {
-        if (NW == 8 && (two_chunks ? ((c0 >> 5) & 1) != half : half != 0)) continue;
         const int ncols = (LEAN || p.BN - c0 >= 32) ? 32 : 16;
         const int n0 = n_base + c0;
         const int nvalid = LEAN ? 32 : min(ncols, p.Cout - n0);
@@ -672,16 +592,15 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sac
     mbar_arrive(tempty_bar);
     acc_phase ^= 1;
   }
-  if (do_stats && cur_img >= 0) flush_stats(cur_img);
 }
 
-template <bool BF16, int NW>
-__device__ __forceinline__ void run_epilogue_direct(const IgemmParams& p, float* sacc, float* sbias, uint64_t* tfull_bar,
-                                                    uint64_t* tempty_bar, const float* accs, int warp, int lane) {
+template <bool BF16>
+__device__ __forceinline__ void run_epilogue_direct(const IgemmParams& p, float* sbias, uint64_t* tfull_bar, uint64_t* tempty_bar,
+                                                    const float* accs, int warp, int lane) {
   const bool lean = (p.flags & IG_GEGLU) && !(p.flags & (IG_OUT_F32_NCHW | IG_RELU | IG_AFFINE_CLAMP01)) && p.out_lo == 0 &&
                     p.res1 == nullptr && p.res2 == nullptr && (p.BN % 32) == 0 && (p.Cout % p.BN) == 0;
-  if (lean) epilogue_direct<BF16, NW, true>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
-  else epilogue_direct<BF16, NW, false>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
+  if (lean) epilogue_direct<BF16, true>(p, sbias, tfull_bar, tempty_bar, accs, warp, lane);
+  else epilogue_direct<BF16, false>(p, sbias, tfull_bar, tempty_bar, accs, warp, lane);
 }
 
 }  // namespace

@@ -22,8 +22,6 @@
 // Warp roles (384 threads, 1 CTA / SM, persistent; see igemm_common.cuh): warps 0..3 epilogue, warps 4..7 the wgmma
 // consumer (and, with XFORM, the operand transform), warp 8 patch producer (two patch slots), warp 11 weight producer
 // (one TMA box per (chunk, tap)).
-#include <cstdlib>
-
 #include "igemm_common.cuh"
 #include "launch.h"
 
@@ -59,12 +57,11 @@ __device__ __forceinline__ void transform_patch(const IgemmParams& p, uint32_t s
   // SWIZZLE_128B: position = logical 16-byte chunk ^ (row & 7); rows advance by 16, so (row & 7) is fixed per thread
   const int jlog = cpos ^ (rbase & 7);             // this thread's logical channel group (8 channels) in every chunk
   const bool do_silu = p.gn_silu != 0;
-  const bool tanh32 = p.gn_silu == 2;              // tanh.approx.f32 instead of the f16x2 form
   const int prows = (p.TH + 2) * kPP;
   const int x0 = t.tx * p.TW - 1, y0 = t.ty * p.TH - 1;
   float sc[8], sh[8];
   const float4* sp = reinterpret_cast<const float4*>(p.gn_ss + (long long)t.z1 * p.gn_C * 2 + (kc * kBK + jlog * 8) * 2);
-  const float pre = (do_silu && !BF16 && !tanh32) ? 0.5f : 1.f;   // the fp16 SiLU form takes h = x / 2: folded into the affine
+  const float pre = (do_silu && !BF16) ? 0.5f : 1.f;   // the fp16 SiLU form takes h = x / 2: folded into the affine
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
     const float4 a = __ldg(sp + e);
@@ -92,7 +89,7 @@ __device__ __forceinline__ void transform_patch(const IgemmParams& p, uint32_t s
       for (int e = 0; e < 4; ++e) {
         float a = fmaf(cvt16<BF16>((uint16_t)(w[u][e] & 0xFFFF)), sc[2 * e], sh[2 * e]);
         float b = fmaf(cvt16<BF16>((uint16_t)(w[u][e] >> 16)), sc[2 * e + 1], sh[2 * e + 1]);
-        if (BF16 || tanh32) {
+        if (BF16) {
           if (do_silu) { a = silu_tanh(a); b = silu_tanh(b); }
           w[u][e] = pack16<BF16>(a, b);
         } else {
@@ -125,7 +122,6 @@ __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* sm
   const int kc_all = p.kc_count + p.kc_sc;
   int slot = 0, stage = 0;
   uint32_t a_phase = 0, b_phase = 0, acc_phase = 0;
-  int mma_n = 0;
   // m64 block mb covers image row mb / 2 of the tile, pixels 64 (mb & 1) ..
   auto row_off = [&](int mb, int dy, int dx) { return ((dy + 1 + (mb >> 1)) * kPP + dx + 1 + (mb & 1) * 64) * 128; };
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -134,15 +130,11 @@ __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* sm
     int held_slot = -1;      // patch slot whose last batch is the one in flight
     for (int kc = 0; kc < kc_all; ++kc) {
       const bool main = kc < p.kc_count;
-      const bool trm = p.trace != nullptr && blockIdx.x == 0 && wc == 0 && lane == 0;
-      const int mix = trm ? mma_n++ : 0;
-      if (trm && mix < 60) p.trace[mix * 8 + 4] = clock64();
       mbar_wait(&a_full[slot], a_phase, 3);                                                   // the patch has landed
       const uint32_t patch = smem_u32(smem + slot * p.a_slot_bytes);
       if constexpr (XFORM) {
         if (main) transform_patch<BF16>(p, patch, t, kc, wc * 32 + lane);
       }
-      if (trm && mix < 60) p.trace[mix * 8 + 5] = clock64();
       const int ntap = main ? 9 : 1;
       for (int tap = 0; tap < ntap; ++tap) {
         const int dy = main ? p.seg[0][tap].dy : 0, dx = main ? p.seg[0][tap].dx : 0;   // shortcut chunk: centre tap only
@@ -173,7 +165,6 @@ __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* sm
         if (++stage == p.stages) { stage = 0; b_phase ^= 1; }
       }
       held_slot = slot;
-      if (trm && mix < 60) p.trace[mix * 8 + 6] = clock64();
       if (++slot == 2) { slot = 0; a_phase ^= 1; }
     }
     wgmma_wait<0>();
@@ -242,8 +233,6 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_patch_kernel(const __gr
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();      // see ptx.cuh: the next kernel may be scheduled; it blocks in its own pdl_wait
-  pdl_wait();         // set-up done; the predecessor grid has completed before any of its outputs is read
 
   // The producer warpgroup gives registers to the other two (igemm_common.cuh).  Each warpgroup's roles sit in their own
   // branch after its setmaxnreg (ptxas ignores a setmaxnreg from which code of a larger budget is reachable); warps 9 and
@@ -252,8 +241,8 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_patch_kernel(const __gr
     setmaxnreg_inc<kWorkerRegs>();
     if (warp < kEpiWarps) {
       // ===================================================================== epilogue
-      if (p.tma_store) run_epilogue_staged<BF16, kEpiWarps, true>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
-      else epilogue_direct<BF16, kEpiWarps, false>(p, sacc, sbias, tfull_bar, tempty_bar, accs, warp, lane);
+      if (p.tma_store) run_epilogue_staged<BF16, true>(p, stg_base, sacc, sbias, tfull_bar, tempty_bar, res_bar, accs, warp, lane);
+      else epilogue_direct<BF16, false>(p, sbias, tfull_bar, tempty_bar, accs, warp, lane);
     } else {
       // ===================================================================== wgmma consumer
       const int wc = warp - kConsumerWarp0;
@@ -317,12 +306,7 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_patch_kernel(const __gr
 
 }  // namespace
 
-static long long* g_patch_trace = nullptr;
-void igemm_patch_set_trace(long long* dev_buf) { g_patch_trace = dev_buf; }
-
-cudaError_t igemm_patch_launch(const IgemmParams& p_in, int grid, cudaStream_t stream) {
-  IgemmParams p = p_in;
-  p.trace = g_patch_trace;
+cudaError_t igemm_patch_launch(const IgemmParams& p, int grid, cudaStream_t stream) {
   static bool attr_set[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);

@@ -3,8 +3,6 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include <cstdlib>
-
 #include "launch.h"
 #include "ptx.cuh"
 
@@ -99,8 +97,6 @@ __device__ __forceinline__ float warp_max(float v) {
 // ------------------------------------------------------------------------------ direct conv
 template <bool BF16>
 __global__ void direct_conv_kernel(const DirectConvParams p) {
-  pdl_trigger();
-  pdl_wait();
   const long long total = (long long)p.N * p.Ho * p.Wo * p.Cout;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -130,7 +126,6 @@ __global__ void direct_conv_kernel(const DirectConvParams p) {
   const long long opix = ((long long)n * p.Ho + oy) * p.Wo + ox;
   if (p.res) acc += load1<BF16>(reinterpret_cast<const uint16_t*>(p.res) + opix * p.out_cstride + co, p.out_lo);
   if (p.flags & DC_RELU) acc = fmaxf(acc, 0.f);
-  if (p.flags & DC_AFFINE_CLAMP01) acc = fminf(fmaxf((acc + 1.f) * 0.5f, 0.f), 1.f);
   if (p.flags & DC_OUT_F32_NCHW) {
     reinterpret_cast<float*>(p.out)[(((long long)n * p.Cout + co) * p.Ho + oy) * p.Wo + ox] = acc;
   } else {
@@ -145,8 +140,6 @@ __global__ void direct_conv_kernel(const DirectConvParams p) {
 template <bool BF16>
 __global__ void gn_stats_kernel(const uint16_t* __restrict__ x, long long HW, int C, float* __restrict__ partial,
                                 int Ctot, int coff, int pix_per_block, int xs, int lo) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ float sh[];   // [PIX][C][2]
   const int n = blockIdx.y;
   const int tid = threadIdx.y * blockDim.x + threadIdx.x;
@@ -197,8 +190,6 @@ __global__ void gn_stats_kernel(const uint16_t* __restrict__ x, long long HW, in
 __global__ void __launch_bounds__(256) gn_finalize_kernel(GnSrc s0, GnSrc s1, int nsrc, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, int N, int Ctot, int groups,
                                                           float inv_count, float eps, float* __restrict__ ss) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ float red[2][8];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x / groups, g = blockIdx.x % groups;
@@ -240,8 +231,6 @@ template <bool BF16, bool SILU>
 __global__ void gn_apply_kernel(const uint16_t* __restrict__ x, long long HW, int C, const float* __restrict__ ss,
                                 int Ctot, int coff, uint16_t* __restrict__ y, int y_cstride, int pix_per_block, int xs,
                                 int lo_x, int lo_y) {
-  pdl_trigger();
-  pdl_wait();
   // blockDim = (C/8 channel vectors, PIX pixel lanes); grid = (pixel chunks, N).  The thread's 8
   // (scale, shift) pairs live in registers for its whole pixel strip.
   const int n = blockIdx.y;
@@ -297,8 +286,6 @@ template <bool BF16, int KV, int TOK>
 __global__ void __launch_bounds__(256) layernorm_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, long long tokens,
                                                         int C, const float* __restrict__ gamma, const float* __restrict__ beta,
                                                         float eps, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const int lane = threadIdx.x & 31;
   const long long tok0 = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * TOK;
   if (tok0 >= tokens) return;
@@ -365,8 +352,6 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const uint16_t* __restri
 constexpr int kSmMaxVec = 8;   // T <= 256 threads * 8 vec * 8 = 16384
 template <bool BF16>
 __global__ void softmax_rows_small_kernel(uint16_t* __restrict__ s, long long rows, int T, int Tp, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const int lane = threadIdx.x & 31;
   const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (r >= rows) return;
@@ -385,8 +370,6 @@ __global__ void softmax_rows_small_kernel(uint16_t* __restrict__ s, long long ro
 // VAE mid-block rows (T = 9216) then hold 24 values per thread instead of 64 (higher occupancy).
 template <bool BF16, int MV>
 __global__ void softmax_rows_kernel(uint16_t* __restrict__ s, int T, int Tp, int lo) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ float red[32];
   uint16_t* row = s + (long long)blockIdx.x * (lo ? 2 * Tp : Tp);
   const int nvec = T / 8;
@@ -442,8 +425,6 @@ constexpr int kSmPipeThreads = 384;
 constexpr int kSmPipeSlots = 3;
 template <bool BF16, int MV>
 __global__ void __launch_bounds__(kSmPipeThreads) softmax_rows_pipe_kernel(uint16_t* __restrict__ s, long long rows, int T, int Tp) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ __align__(128) uint8_t sm_raw[];
   __shared__ float red[2][kSmPipeThreads / 32];
   __shared__ __align__(8) uint64_t full[kSmPipeSlots];
@@ -536,8 +517,6 @@ template <bool BF16, int KV, int TOK>
 __global__ void xattn2_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, long long tokens, int C,
                               int heads, const float* __restrict__ U, const float* __restrict__ u0,
                               const float* __restrict__ M, const float* __restrict__ c0, float eps, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const int lane = threadIdx.x & 31;
   const long long tok0 = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * TOK;
   if (tok0 >= tokens) return;
@@ -645,8 +624,6 @@ __global__ void __launch_bounds__(KV >= 5 ? 512 : 256) xattn2_smem_kernel(const 
                                                           int C, int heads, const float* __restrict__ U,
                                                           const float* __restrict__ u0, const float* __restrict__ M,
                                                           const float* __restrict__ c0, float eps, int lo) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ __align__(16) float xa_sm[];
   float* sU = xa_sm;
   float* sM = sU + heads * C;
@@ -772,28 +749,8 @@ __global__ void __launch_bounds__(KV >= 5 ? 512 : 256) xattn2_smem_kernel(const 
 
 // ------------------------------------------------------------------------------ elementwise
 template <bool BF16>
-__global__ void geglu_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, long long total_vec, int C4) {
-  pdl_trigger();
-  pdl_wait();
-  const int nvec = C4 / 8;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total_vec;
-       i += (long long)gridDim.x * blockDim.x) {
-    const long long tok = i / nvec;
-    const int v = (int)(i % nvec);
-    float a[8], g[8];
-    unpack8<BF16>(__ldg(reinterpret_cast<const uint4*>(in + tok * 2 * C4 + v * 8)), a);
-    unpack8<BF16>(__ldg(reinterpret_cast<const uint4*>(in + tok * 2 * C4 + C4 + v * 8)), g);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) a[e] *= 0.5f * g[e] * (1.f + erff(g[e] * 0.70710678118654752f));
-    *reinterpret_cast<uint4*>(out + tok * C4 + v * 8) = pack8<BF16>(a);
-  }
-}
-
-template <bool BF16>
 __global__ void relu_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, long long total_vec, int nvec,
                             int lo) {
-  pdl_trigger();
-  pdl_wait();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total_vec;
        i += (long long)gridDim.x * blockDim.x) {
     const long long off = lo ? (i / nvec) * (2LL * lo) + (i % nvec) * 8 : i * 8;   // [pixel][hi C | lo C]
@@ -808,8 +765,6 @@ __global__ void relu_kernel(const uint16_t* __restrict__ in, uint16_t* __restric
 template <bool BF16>
 __global__ void bilinear_up2x_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, int N, int H, int W,
                                      int C, float sy, float sx, long long total_vec, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const int nvec = C / 8;
   const int Ho = 2 * H, Wo = 2 * W;
   const int xs = lo ? 2 * C : C;
@@ -837,26 +792,6 @@ __global__ void bilinear_up2x_kernel(const uint16_t* __restrict__ in, uint16_t* 
   }
 }
 
-template <bool BF16>
-__global__ void preprocess_kernel(const void* __restrict__ in, int kind, uint16_t* __restrict__ out, int N,
-                                  long long HW, int lo) {
-  pdl_trigger();
-  pdl_wait();
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)N * HW) return;
-  const int n = (int)(i / HW);
-  const long long p = i % HW;
-  float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const long long off = ((long long)n * 3 + c) * HW + p;
-    if (kind == 0) f[c] = (float)reinterpret_cast<const uint8_t*>(in)[off] / 255.0f * 2.0f - 1.0f;
-    else if (kind == 1) f[c] = f16_to_f32<false>(reinterpret_cast<const uint16_t*>(in)[off]);
-    else f[c] = reinterpret_cast<const float*>(in)[off];
-  }
-  store8<BF16>(out + i * (lo ? 16 : 8), lo, f);
-}
-
 // K-packed stem: the 3x3 neighbourhood of every pixel laid out along the channel axis, NHWC32 =
 // [centre tap (3 ch) | the other 8 taps in row-major order (24 ch) | 5 zeros], so that AutoencoderKL.encoder.conv_in
 // (3 -> 128, 3x3) becomes a 1x1 GEMM with K = 27 (one 64-channel chunk) instead of nine 64-wide chunks of which 3
@@ -864,8 +799,6 @@ __global__ void preprocess_kernel(const void* __restrict__ in, int kind, uint16_
 template <bool BF16>
 __global__ void preprocess_im2col_kernel(const void* __restrict__ in, int kind, uint16_t* __restrict__ out, int N, int H, int W,
                                          int lo) {
-  pdl_trigger();
-  pdl_wait();
   const long long HW = (long long)H * W;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)N * HW) return;
@@ -909,14 +842,10 @@ __device__ __forceinline__ float ord2f(unsigned int u) {
   return __uint_as_float((u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u);
 }
 __global__ void minmax_init_kernel(unsigned int* s, int N) {
-  pdl_trigger();
-  pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < N) { s[2 * i] = 0xFFFFFFFFu; s[2 * i + 1] = 0u; }
 }
 __global__ void minmax_reduce_kernel(const float* __restrict__ x, long long HW, unsigned int* s) {
-  pdl_trigger();
-  pdl_wait();
   const int n = blockIdx.y;
   float mn = INFINITY, mx = -INFINITY;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x) {
@@ -927,8 +856,6 @@ __global__ void minmax_reduce_kernel(const float* __restrict__ x, long long HW, 
   if ((threadIdx.x & 31) == 0) { atomicMin(&s[2 * n], f2ord(mn)); atomicMax(&s[2 * n + 1], f2ord(mx)); }
 }
 __global__ void minmax_apply_kernel(float* __restrict__ x, long long HW, const unsigned int* __restrict__ s, float dmin, int zero_min) {
-  pdl_trigger();
-  pdl_wait();
   const int n = blockIdx.y;
   const float mn = zero_min ? 0.f : ord2f(s[2 * n]), mx = ord2f(s[2 * n + 1]);
   const float d = fmaxf(mx - mn, dmin);
@@ -1048,8 +975,7 @@ cudaError_t softmax_rows(void* sio, long long rows, int T, int Tp, bool bf16, cu
     return cudaGetLastError();
   }
   if (T / 8 > 256 * kSmMaxVec) return cudaErrorInvalidValue;
-  static const bool no_pipe = [] { const char* e = getenv("GP_SOFTMAX_PIPE"); return e && e[0] == '0'; }();
-  if (!split && !no_pipe && T >= 2048 && T / 8 <= kSmPipeThreads * 6 && rows >= 1024) {
+  if (!split && T >= 2048 && T / 8 <= kSmPipeThreads * 6 && rows >= 1024) {
     const int slot_bytes = (T * 2 + 127) & ~127;
     const int smem = kSmPipeSlots * slot_bytes;
     if (smem <= 200 * 1024) {
@@ -1103,9 +1029,8 @@ cudaError_t xattn2(const void* x, void* y, long long tokens, int C, int heads, c
   if (C % 8 || C / 8 > 32 * kLnMaxVec) return cudaErrorInvalidValue;
   const int kv = (C / 8 + 31) / 32;
   cudaError_t e = cudaSuccess;
-  static const bool no_smem = [] { const char* v = getenv("GP_XATTN_SMEM"); return v && v[0] == '0'; }();
   const size_t smem = ((size_t)2 * heads * C + C + heads) * sizeof(float);
-  if (!no_smem && heads % kXaHB == 0 && C % 32 == 0 && smem <= 226 * 1024) {
+  if (heads % kXaHB == 0 && C % 32 == 0 && smem <= 226 * 1024) {
     static int sms[64] = {0};
     int dev = 0;
     cudaGetDevice(&dev);
@@ -1143,13 +1068,6 @@ cudaError_t xattn2(const void* x, void* y, long long tokens, int C, int heads, c
   return e;
 }
 
-cudaError_t geglu(const void* in, void* out, long long tokens, int C4, bool bf16, cudaStream_t s) {
-  const long long total_vec = tokens * (C4 / 8);
-  GP_DISPATCH_BF16(bf16, (launch(geglu_kernel<BF>, blocks_for(total_vec, 256), 256, 0, s, 
-                             reinterpret_cast<const uint16_t*>(in), reinterpret_cast<uint16_t*>(out), total_vec, C4)));
-  return cudaGetLastError();
-}
-
 cudaError_t relu16(const void* in, void* out, long long n, bool bf16, cudaStream_t s, int split_c) {
   const long long total_vec = n / 8;        // n = pixels * C logical elements
   GP_DISPATCH_BF16(bf16, (launch(relu_kernel<BF>, blocks_for(total_vec, 256), 256, 0, s, 
@@ -1168,20 +1086,10 @@ cudaError_t bilinear_up2x(const void* in, void* out, int N, int H, int W, int C,
   return cudaGetLastError();
 }
 
-cudaError_t preprocess_rgb(const void* in, int in_kind, void* out, int N, int H, int W, bool bf16, cudaStream_t s, bool split) {
-  const long long HW = (long long)H * W;
-  const long long total = (long long)N * HW;
-  GP_DISPATCH_BF16(bf16, (launch(preprocess_kernel<BF>, (unsigned)((total + 255) / 256), 256, 0, s, 
-                             in, in_kind, reinterpret_cast<uint16_t*>(out), N, HW, split ? 8 : 0)));
-  return cudaGetLastError();
-}
-
 namespace {
 // 16-bit NHWC8 (first `c` channels) -> fp32 NCHW [N, c, H, W]
 template <bool BF16>
 __global__ void nhwc8_to_nchw_kernel(const uint16_t* __restrict__ in, float* __restrict__ out, int N, long long HW, int c, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)N * HW) return;
   const int n = (int)(i / HW);
@@ -1197,8 +1105,6 @@ __global__ void nhwc8_to_nchw_kernel(const uint16_t* __restrict__ in, float* __r
 template <bool BF16>
 __global__ void nchw4_affine_to_nhwc8_kernel(const float* __restrict__ in, uint16_t* __restrict__ out, int N, long long HW,
                                              float pre, const float* __restrict__ m, const float* __restrict__ b, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)N * HW) return;
   const int n = (int)(i / HW);
@@ -1227,8 +1133,6 @@ namespace {
 template <bool BF16>
 __global__ void latent_pack_kernel(const uint16_t* __restrict__ lat, const uint16_t* __restrict__ smp, uint16_t* __restrict__ xin,
                                    long long npx, int in_ch, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npx) return;
   const long long o = i * (lo ? 16 : 8);
@@ -1249,8 +1153,6 @@ __global__ void latent_pack_kernel(const uint16_t* __restrict__ lat, const uint1
 template <bool BF16>
 __global__ void ddim_step_kernel(const uint16_t* __restrict__ mo, uint16_t* __restrict__ smp, uint16_t* __restrict__ x0, long long npx,
                                  float c0, float c1, float c2, float c3, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npx) return;
   const long long o = i * (lo ? 16 : 8);
@@ -1269,8 +1171,6 @@ __global__ void ddim_step_kernel(const uint16_t* __restrict__ mo, uint16_t* __re
 template <bool BF16>
 __global__ void latent_affine_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, long long npx, float pre,
                                      const float* __restrict__ mat, const float* __restrict__ bias, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npx) return;
   const long long o = i * (lo ? 16 : 8);
@@ -1344,8 +1244,6 @@ namespace {
 // median (torch.median: the LOWER middle value for an even count) or mean.
 __global__ void ensemble_reduce_kernel(const float* __restrict__ d, int B, long long HW, const float* __restrict__ sc,
                                        const float* __restrict__ sh, int median, float* __restrict__ out) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= HW) return;
   float v[32];
@@ -1371,8 +1269,6 @@ cudaError_t ensemble_reduce(const float* d, int B, long long HW, const float* sc
 namespace {
 __global__ void nearest_resize_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, int N, int H, int W, int OH,
                                       int OW, int nvec, float sy, float sx, long long total_vec) {
-  pdl_trigger();
-  pdl_wait();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total_vec;
        i += (long long)gridDim.x * blockDim.x) {
     const int v = (int)(i % nvec);
@@ -1390,8 +1286,6 @@ __global__ void nearest_resize_kernel(const uint4* __restrict__ in, uint4* __res
 namespace {
 template <bool BF16>
 __global__ void softmax_groups_kernel(uint16_t* __restrict__ x, long long rows, int ld, int groups, int n, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * groups) return;
   uint16_t* p = x + (i / groups) * (lo ? 2 * ld : ld) + (i % groups) * n;
@@ -1417,8 +1311,6 @@ namespace {
 template <bool BF16>
 __global__ void bilinear_resize_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, int N, int H, int W, int OH,
                                        int OW, int C, float sy, float sx, long long total_vec, int lo) {
-  pdl_trigger();
-  pdl_wait();
   const int nvec = C / 8;
   const int xs = lo ? 2 * C : C;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total_vec;

@@ -1,5 +1,5 @@
 // Bandwidth-bound and small kernels of the hot path (everything that is not a dense contraction):
-// GroupNorm(+SiLU), LayerNorm, row softmax, the 2-token cross-attention closed form, GEGLU,
+// GroupNorm(+SiLU), LayerNorm, row softmax, the 2-token cross-attention closed form,
 // ReLU, bilinear 2x, direct convolution for tiny channel counts (and as the on-device triage
 // reference for the wgmma kernels), pre/post-processing.  16-bit NHWC activations, fp32 math.
 // `split` = the high-precision layout: C logical channels stored as [hi C | lo C] per pixel (two fp16 planes,
@@ -13,7 +13,6 @@ namespace gp {
 enum DirectConvFlags : int {
   DC_RELU = 1,
   DC_OUT_F32_NCHW = 2,
-  DC_AFFINE_CLAMP01 = 4,
   DC_UP2X = 8,          // input is nearest-2x upsampled before the convolution
 };
 
@@ -52,7 +51,6 @@ cudaError_t softmax_rows(void* s_inout, long long rows, int T, int Tp, bool bf16
 cudaError_t xattn2(const void* x, void* y, long long tokens, int C, int heads, const float* U /*[h][C]*/,
                    const float* u0 /*[h]*/, const float* M /*[h][C]*/, const float* c0 /*[C]*/,
                    float eps, bool bf16, cudaStream_t s, bool split = false);
-cudaError_t geglu(const void* in, void* out, long long tokens, int C4, bool bf16, cudaStream_t s);
 // split_c: 0, or the logical channel count C of a high-precision [hi C | lo C] tensor (n = pixels * C)
 cudaError_t relu16(const void* in, void* out, long long n, bool bf16, cudaStream_t s, int split_c = 0);
 cudaError_t bilinear_up2x(const void* in, void* out, int N, int H, int W, int C, bool bf16,
@@ -67,17 +65,15 @@ cudaError_t nearest_resize(const void* in, void* out, int N, int H, int W, int O
 // skip feature to the running map's size, /root/reference/genpercept/models/dpt_head.py:297-300)
 cudaError_t bilinear_resize(const void* in, void* out, int N, int H, int W, int OH, int OW, int C, bool bf16, cudaStream_t s,
                             bool split = false);
-// u8 / f16 / f32 NCHW [N,3,H,W] -> 16-bit NHWC8 (channels 3..7 zero); u8 is mapped x/255*2-1.
-cudaError_t preprocess_rgb(const void* in, int in_kind /*0 u8, 1 f16, 2 f32*/, void* out, int N, int H,
-                           int W, bool bf16, cudaStream_t s, bool split = false);
 // latent I/O of encode_rgb / decode_pred: 16-bit NHWC8 <-> fp32 NCHW [N,4,H,W]; the second form applies
 // y = M (x * pre) + b per pixel (post_quant_conv(latent / 0.18215), genpercept_pipeline.py:519-521)
 cudaError_t nhwc8_to_nchw_f32(const void* in, float* out, int N, int H, int W, int c, bool bf16, cudaStream_t s, bool split = false);
 cudaError_t nchw4_affine_to_nhwc8(const float* in, void* out, int N, int H, int W, float pre, const float* m /*[4][4] or null*/,
                                   const float* b /*[4] or null*/, bool bf16, cudaStream_t s, bool split = false);
-// Same input as preprocess_rgb, K-packed for the VAE encoder's stem: 16-bit NHWC32 = the pixel's 3x3 neighbourhood along
-// the channel axis [centre tap | 8 other taps row-major | 5 zeros]; im2col_tap_slot(r, q) gives a tap's position.
-cudaError_t preprocess_rgb_im2col(const void* in, int in_kind, void* out, int N, int H, int W, bool bf16, cudaStream_t s,
+// u8 / f16 / f32 NCHW [N,3,H,W] (u8 is mapped x/255*2-1), K-packed for the VAE encoder's stem: 16-bit NHWC32 = the pixel's
+// 3x3 neighbourhood along the channel axis [centre tap | 8 other taps row-major | 5 zeros]; im2col_tap_slot(r, q) gives a
+// tap's position.
+cudaError_t preprocess_rgb_im2col(const void* in, int in_kind /*0 u8, 1 f16, 2 f32*/, void* out, int N, int H, int W, bool bf16, cudaStream_t s,
                                   bool split = false);
 inline int im2col_tap_slot(int r, int q) {      // 3x3 tap (r, q) -> group of 3 channels inside the NHWC32 pixel
   if (r == 1 && q == 1) return 0;

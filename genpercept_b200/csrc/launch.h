@@ -1,17 +1,8 @@
-// Kernel launch helper: cudaLaunchKernelEx, optionally with the programmatic-dependent-launch attribute (see ptx.cuh,
-// pdl_wait).  Opt-in (GP_PDL=1): inside a CUDA graph the launch gaps are already short and the early-resident CTAs
-// only add scheduling work.
+// Kernel launch helper: the one launch idiom of the engine (cudaLaunchKernelEx with the kernel's argument types).
 #pragma once
 #include <cuda_runtime.h>
 
-#include <cstdlib>
-
 namespace gp {
-
-inline bool pdl_enabled() {
-  static const bool on = [] { const char* e = getenv("GP_PDL"); return e && e[0] == '1'; }();
-  return on;
-}
 
 template <typename... P, typename... A>
 inline cudaError_t launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A&&... args) {
@@ -20,11 +11,6 @@ inline cudaError_t launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t sm
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<P>(args)...);
 }
 

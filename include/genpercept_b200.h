@@ -183,14 +183,6 @@ gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, v
 /* time one igemm configuration: returns average microseconds over `iters` launches */
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters,
                         double* usec, double* flops);
-/* debug: a device buffer of >= 512 int64 that CTA 0 of the fused-attention launches planned afterwards fills with
- * clock64() stamps, slots 8j + {0, 1, 2} of key block j < 64: block start, S = Q K^T done, O += P V done (thread 0);
- * NULL switches the stamps off again. */
-void gp_debug_fattn_trace(void* dev_buf);
-/* debug: a device buffer of >= 512 int64 that CTA 0 of the patch-resident kernel launches made afterwards fills with
- * clock64() stamps, slots 8k + {4, 5, 6} of K chunk k < 60 (wgmma consumer: before the patch wait / patch ready, after
- * the GroupNorm transform if any / all taps issued and retired); NULL switches the stamps off. */
-void gp_debug_patch_trace(void* dev_buf);
 
 #ifdef __cplusplus
 }
