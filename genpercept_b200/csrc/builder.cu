@@ -8,8 +8,17 @@
 
 #include "engine.h"
 #include "fattn.h"
+#include "fattn512.h"
 
 namespace gp {
+
+// Single-head d = 512 attention (the VAE mid-block) takes the fused kernel (fattn512.cu) once the unfused path's score
+// matrix S would exceed this many bytes, or where the unfused path cannot run at all (rows longer than softmax_rows
+// takes).  Below it the unfused path (QK^T GEMM -> softmax -> P V GEMM) is kept: it is what every size up to and
+// including bench.py's largest configuration (8 x 768^2: 1.36 GB of S) has always run, so those outputs stay
+// bit-identical.  Above it S alone decides whether a photo fits on the card (49 GB at 2592 x 3872), while the fused
+// kernel needs no workspace at all.
+constexpr size_t kFusedAttnMinBytes = size_t(2) << 30;
 
 // ------------------------------------------------------------------------------------ Arena
 size_t Arena::alloc(size_t bytes) {
@@ -519,6 +528,29 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
     return;
   }
   const size_t s_bytes = (size_t)B * heads * T * TpP * 2;
+  // the unfused path's softmax_rows cannot take rows past kSoftmaxRowsMaxT keys when T is a multiple of 8
+  const bool unfused_runs = T % 8 != 0 || T <= kSoftmaxRowsMaxT;
+  const bool fused512 = d == 512 && heads == 1 && !split_ &&
+                        (attn512_path >= 0 ? attn512_path == 1 : s_bytes > kFusedAttnMinBytes || !unfused_runs);
+  if (fused512) {   // fused d = 512 kernel: no score matrix in the arena
+    if (measuring_) return;
+    Fattn512Params p;
+    std::memset(&p, 0, sizeof(p));
+    p.out = ptr(out);
+    p.bias = pv_bias;
+    p.out_b_stride = (long long)T * out.ps();
+    p.out_row_stride = (int)out.ps();
+    p.T = T; p.B = B; p.q_tiles = ceil_div(T, 64);
+    p.scale_log2e = 1.4426950408889634f;
+    p.bf16 = bf16_ ? 1 : 0;
+    check_cuda(make_tmap_b(&p.tmQ, q, C, T, B, cs, (long long)T * cs, 64, bf16_), name + ": tmap Q");
+    check_cuda(make_tmap_b(&p.tmK, k, C, T, B, cs, (long long)T * cs, 64, bf16_), name + ": tmap K");
+    check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, Tp, (long long)C * Tp, 64, bf16_), name + ": tmap Vt");
+    push(name + ".fattn512", 1, 4.0 * B * (double)T * T * d, 4.0 * B * T * C * 2,
+         [p](cudaStream_t s) { return fattn512_launch(p, s); });
+    ops.back().kind = 2;
+    return;
+  }
   const size_t s_off = arena_.alloc(s_bytes);
   if (!measuring_) {
     void* S = raw_ptr(s_off);

@@ -1201,7 +1201,16 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
     std::unique_ptr<Plan> p(new Plan());
     p->B = B; p->H = H; p->W = W;
     p->arena_bytes = m.arena_bytes();
-    GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->arena), p->arena_bytes));
+    const cudaError_t ae = cudaMalloc(reinterpret_cast<void**>(&p->arena), p->arena_bytes);
+    if (ae == cudaErrorMemoryAllocation) {
+      // Not a sticky error: clear it and report the shape as too large, so the engine stays usable for smaller inputs.
+      cudaGetLastError();
+      p->arena = nullptr;
+      throw GpError(GP_ERR_INVALID, "gp_plan: batch " + std::to_string(B) + " at " + std::to_string(H) + "x" +
+                                        std::to_string(W) + " needs an activation arena of " +
+                                        std::to_string(p->arena_bytes) + " bytes, more than the device can allocate");
+    }
+    GP_CUDA(ae);
     GP_CUDA(cudaMemset(p->arena, 0, p->arena_bytes));
     Builder b(e->bf16, false, p->arena, e->split);
     e->build(b, p.get(), B, H, W);
@@ -1865,6 +1874,68 @@ gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int k
     cudaEventDestroy(e1);
     if (usec) *usec = ms * 1000.0 / iters;
     if (flops) *flops = b.ops[0].flops;
+  });
+}
+
+gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, double* usec, double* flops) {
+  return guarded_free([&]() {
+    GP_REQUIRE(dtype == GP_F16 || dtype == GP_BF16, "gp_bench_attention: dtype must be f16/bf16");
+    GP_REQUIRE(B >= 1 && T >= 1 && iters >= 1, "gp_bench_attention: bad arguments");
+    TempEngine te(dtype);
+    const int C = 512;
+    const int Tp = (T + 7) / 8 * 8;
+    // The VAE mid-block's operands: q | k packed at a pixel stride of 2C, V^T [B][C][Tp], out [B][T][C].
+    const size_t qk_n = (size_t)B * T * 2 * C, vt_n = (size_t)B * C * Tp, o_n = (size_t)B * T * C;
+    void *qk = nullptr, *vT = nullptr, *o = nullptr, *arena = nullptr;
+    GP_CUDA(cudaMalloc(&qk, qk_n * 2));
+    te.e.dev_allocs.push_back(qk);
+    GP_CUDA(cudaMalloc(&vT, vt_n * 2));
+    te.e.dev_allocs.push_back(vT);
+    GP_CUDA(cudaMalloc(&o, o_n * 2));
+    te.e.dev_allocs.push_back(o);
+    // Small pseudo-random operands (scores of order one, as in the model) rather than zeros, so the tensor cores switch
+    // as they do on real data.
+    {
+      std::vector<uint16_t> pat((size_t)1 << 20);
+      uint32_t x = 12345u;
+      for (auto& v : pat) {
+        x = x * 1664525u + 1013904223u;
+        const float f = ((int)(x >> 9) - (1 << 22)) * (0.3f / (1 << 22));
+        v = host_f2h(f, te.e.bf16);
+      }
+      for (auto [buf, n] : {std::make_pair(qk, qk_n), std::make_pair(vT, vt_n)})
+        for (size_t i = 0; i < n; i += pat.size())
+          GP_CUDA(cudaMemcpy(reinterpret_cast<uint16_t*>(buf) + i, pat.data(), std::min(pat.size(), n - i) * 2,
+                             cudaMemcpyHostToDevice));
+    }
+    {
+      Builder m(te.e.bf16, true, nullptr);
+      m.attn512_path = fused ? 1 : 0;
+      m.attention_qkv("a", nullptr, nullptr, 2 * C, nullptr, B, T, 1, C, nullptr, T4{});
+      if (m.arena_bytes()) {
+        GP_CUDA(cudaMalloc(&arena, m.arena_bytes()));
+        te.e.dev_allocs.push_back(arena);
+      }
+    }
+    Builder b(te.e.bf16, false, reinterpret_cast<uint8_t*>(arena));
+    b.attn512_path = fused ? 1 : 0;
+    b.attention_qkv("attn", qk, reinterpret_cast<uint16_t*>(qk) + C, 2 * C, vT, B, T, 1, C, nullptr,
+                    b.external(o, B, 1, T, C));
+    cudaEvent_t e0, e1;
+    GP_CUDA(cudaEventCreate(&e0));
+    GP_CUDA(cudaEventCreate(&e1));
+    run_all(b, 0);
+    GP_CUDA(cudaDeviceSynchronize());
+    GP_CUDA(cudaEventRecord(e0, 0));
+    for (int i = 0; i < iters; ++i) run_all(b, 0);
+    GP_CUDA(cudaEventRecord(e1, 0));
+    GP_CUDA(cudaEventSynchronize(e1));
+    float ms = 0;
+    GP_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    if (usec) *usec = ms * 1000.0 / iters;
+    if (flops) *flops = 4.0 * B * (double)T * T * C;
   });
 }
 

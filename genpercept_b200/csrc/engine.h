@@ -155,6 +155,9 @@ class Builder {
   // When set, ops that write the final fp32 map (ConvArgs::out_f32 / direct(..., out_f32)) read their destination from
   // *out_slot at LAUNCH time, so gp_infer can point them at the caller's device buffer (no copy of the result).
   float** out_slot = nullptr;
+  // Single-head d = 512 attention path: -1 chooses by the size of the score matrix (kFusedAttnMinBytes, builder.cu);
+  // 0 forces the unfused path, 1 the fused kernel.  Only gp_bench_attention sets it, to time both paths at one shape.
+  int attn512_path = -1;
 
  private:
   void push(const std::string& name, int launches, double flops, double bytes,

@@ -350,6 +350,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const uint16_t* __restri
 
 // ------------------------------------------------------------------------------ row softmax
 constexpr int kSmMaxVec = 8;   // T <= 256 threads * 8 vec * 8 = 16384
+static_assert(256 * kSmMaxVec * 8 == kSoftmaxRowsMaxT, "kernels.h states the row limit");
 template <bool BF16>
 __global__ void softmax_rows_small_kernel(uint16_t* __restrict__ s, long long rows, int T, int Tp, int lo) {
   const int lane = threadIdx.x & 31;

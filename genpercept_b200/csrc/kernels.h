@@ -45,7 +45,9 @@ cudaError_t gn_apply(const void* x, int N, long long HW, int C, const float* sca
 
 cudaError_t layernorm(const void* x, void* y, long long tokens, int C, const float* gamma,
                       const float* beta, float eps, bool bf16, cudaStream_t s, bool split = false);
-// in-place softmax over the first T entries of each row (row stride Tp elements)
+// in-place softmax over the first T entries of each row (row stride Tp elements).  Where T is a multiple of 8 (and
+// >= 64) rows are limited to kSoftmaxRowsMaxT entries (cudaErrorInvalidValue beyond); other T have no limit.
+constexpr int kSoftmaxRowsMaxT = 16384;
 cudaError_t softmax_rows(void* s_inout, long long rows, int T, int Tp, bool bf16, cudaStream_t s, bool split = false);
 // y = x + c0 + sigmoid(LN(x) . U + u0) . M     (SURVEY.md F6; U already carries LN gamma, u0 beta)
 cudaError_t xattn2(const void* x, void* y, long long tokens, int C, int heads, const float* U /*[h][C]*/,

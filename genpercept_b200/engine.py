@@ -78,6 +78,7 @@ def lib():
     L.gp_bilinear_up2x.argtypes = [c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
     L.gp_bench_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_double),
                                 POINTER(c_double)]
+    L.gp_bench_attention.argtypes = [c_int, c_int, c_int, c_int, c_int, POINTER(c_double), POINTER(c_double)]
     L.gp_resize_aa.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
                                c_int, c_void_p]
     L.gp_colorize.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_int,
@@ -442,4 +443,13 @@ def bench_conv(dtype, N, H, W, Cin, Cout, ks=3, mode=0, iters=10):
     us, fl = c_double(), c_double()
     st = lib().gp_bench_conv(_gp_dtype(dtype), N, H, W, Cin, Cout, ks, mode, iters, byref(us), byref(fl))
     _check_free(st, "gp_bench_conv")
+    return us.value, fl.value
+
+
+def bench_attention(dtype, B, T, fused, iters=10):
+    """Time the fused or the unfused single-head d = 512 attention (VAE mid-block) at B x T tokens, whichever path the
+    planner would choose there.  Returns (microseconds per call, FLOPs per call)."""
+    us, fl = c_double(), c_double()
+    st = lib().gp_bench_attention(_gp_dtype(dtype), B, T, 1 if fused else 0, iters, byref(us), byref(fl))
+    _check_free(st, "gp_bench_attention")
     return us.value, fl.value

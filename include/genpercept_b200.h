@@ -183,6 +183,10 @@ gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, v
 /* time one igemm configuration: returns average microseconds over `iters` launches */
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters,
                         double* usec, double* flops);
+/* time one path of the single-head d = 512 attention (the VAE mid-block) on B images of T tokens: fused != 0 the fused
+ * kernel, 0 the unfused QK^T -> softmax -> P V path, whichever the planner would pick for that size.  Returns the
+ * average microseconds over `iters` calls after one warm-up call, and the algorithmic FLOPs (4 B T^2 512) of one call. */
+gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, double* usec, double* flops);
 
 #ifdef __cplusplus
 }
