@@ -112,7 +112,6 @@ void Builder::custom(const std::string& name, int launches, double bytes, std::f
   push(name, launches, 0, bytes, std::move(fn));
 }
 
-static int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // N tile: one of the wgmma widths the GEMM kernels are built for (16, 32, 64, 128).  Cout = 320 (the SD-2.1 UNet's first
 // level) takes 64 (five exact tiles): a multiple of 64 keeps the staged TMA-store epilogue.
 int choose_bn(int cout, int force) {
@@ -221,10 +220,7 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   if (gn_fused) gn_scale_shift(a.gn_name, a.srcs, *a.gn, a.gn_groups, a.gn_eps);
   const T4& s0 = a.srcs[0];
   const int N = s0.N, H = s0.H, W = s0.W;
-  int Ho = H, Wo = W;
-  if (a.mode == 1) { Ho = (H + 2 - 3) / 2 + 1; Wo = (W + 2 - 3) / 2 + 1; }
-  if (a.mode == 2) { Ho = (H + 1 - 3) / 2 + 1; Wo = (W + 1 - 3) / 2 + 1; }
-  if (a.mode == 3) { Ho = 2 * H; Wo = 2 * W; }
+  const auto [Ho, Wo] = conv_out_dims(a.mode, H, W);
   const int PL = split_ ? 2 : 1;
   const int out_cl = a.out_f32 ? 0 : a.out.C;   // logical channels of the 16-bit output ...
   const int out_c = out_cl * PL;                // ... and its pixel stride in elements
@@ -495,6 +491,13 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   if (a.mode == 3) ops.back().flops_exec = flops * 4.0 / 9.0;      // four 2x2 parity convs instead of a 3x3 on the 2x grid
 }
 
+// The high-precision mode's three GEMM passes: hi*hi + lo*hi + hi*lo (A planes at tmA[0] / tmA[4], B at tmB / tmB2)
+static void set_passes(IgemmParams& p) {
+  p.npass = 3;
+  p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
+  p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = 1;
+}
+
 void Builder::attention_qkv(const std::string& name, const void* q, const void* k, long long cs, const void* vT, int B,
                             int T, int heads, int d, const float* pv_bias, const T4& out, long long qk_lo) {
   // High-precision mode: q / k carry their lo planes `qk_lo` elements further (same pixel stride cs), V^T rows are
@@ -503,12 +506,6 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
   const int C = heads * d;
   const int PL = split_ ? 2 : 1;
   const long long TpP = (long long)Tp * PL;   // physical row pitch of S and V^T
-  auto set_passes = [&](IgemmParams& p) {
-    if (!split_) return;
-    p.npass = 3;
-    p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
-    p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = 1;
-  };
   if (d == 64 && !split_) {   // fused wgmma flash-attention kernel (S and P stay on chip)
     if (measuring_) return;
     FattnParams p;
@@ -644,49 +641,55 @@ void Builder::attention(const std::string& name, const T4& l, const PackedW& wqk
   const int PL = split_ ? 2 : 1;
   const long long TpP = (long long)Tp * PL;
   GP_REQUIRE(wv.planes == PL && wqk.planes == PL, name + ": packed weights do not match the engine's precision mode");
-  const size_t vt_bytes = (size_t)B * C * TpP * 2;
-  const size_t vt_off = arena_.alloc(vt_bytes);
-  if (!measuring_) {   // V^T[b] = Wv . l[b]^T : A = weights (rows = channels), B = tokens
-    IgemmParams p;
-    std::memset(&p, 0, sizeof(p));
-    p.flags = bf16_ ? IG_BF16 : 0;
-    p.gridW = C; p.gridH = 1; p.TW = 128; p.TH = 1; p.tw_shift = 7;
-    p.Z1 = B; p.Z0 = 1;
-    p.b_z_z1 = 1;
-    p.nseg[0] = 1;
-    p.seg[0][0] = IgemmSeg{0, 0, 0, (uint16_t)(wv.ktot / 64)};
-    p.out = raw_ptr(vt_off); p.outW = C; p.outH = 1;
-    p.out_pix_stride = TpP; p.out_row_stride = 0;
-    p.out_z1 = (long long)C * TpP;
-    p.out_sy = p.out_sx = 1;
-    p.Cout = T;
-    p.BN = choose_bn(T, 0);
-    const long long wrow = (long long)wv.ktot * PL;
-    check_cuda(make_tmap_a(&p.tmA[0], wv.w, wv.ktot, C, 1, 1, wrow, (long long)C * wrow, (long long)C * wrow,
-                           128, 1, bf16_), name + ": tmap Wv");
-    for (int i = 1; i < 4; ++i) p.tmA[i] = p.tmA[0];
-    check_cuda(make_tmap_b(&p.tmB, ptr(l), C, T, B, l.ps(), (long long)T * l.ps(), p.BN, bf16_), name + ": tmap l");
-    if (split_) {
-      check_cuda(make_tmap_a(&p.tmA[4], wv.w + wv.ktot, wv.ktot, C, 1, 1, wrow, (long long)C * wrow, (long long)C * wrow,
-                             128, 1, bf16_), name + ": tmap Wv lo");
-      for (int i = 5; i < 8; ++i) p.tmA[i] = p.tmA[4];
-      check_cuda(make_tmap_b(&p.tmB2, reinterpret_cast<const uint16_t*>(ptr(l)) + C, C, T, B, l.ps(), (long long)T * l.ps(), p.BN, bf16_),
-                 name + ": tmap l lo");
-      p.npass = 3;
-      p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
-      p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = 1;
-      p.out_lo = Tp;
-    }
-    finalize_or_throw(&p, name + ".to_vT");
-    push(name + ".to_vT", 1, 2.0 * B * (double)T * C * C, (double)vt_bytes + (double)l.bytes(),
-         [p](cudaStream_t s) { return igemm_launch(p, s); });
-    ops.back().kind = 1;
-  }
+  const size_t vt_off = arena_.alloc((size_t)B * C * TpP * 2);
+  to_vT(name, l, wv, measuring_ ? nullptr : raw_ptr(vt_off));
   const uint16_t* qp = measuring_ ? nullptr : reinterpret_cast<const uint16_t*>(ptr(qk));
   attention_qkv(name, qp, qp ? qp + C : nullptr, qk.ps(), measuring_ ? nullptr : raw_ptr(vt_off), B, T, heads, d, pv_bias, out,
                 split_ ? 2LL * C : 0);
   arena_.release(vt_off);
   release(qk);
+}
+
+void Builder::to_vT(const std::string& name, const T4& l, const PackedW& wv, void* vT) {
+  if (measuring_) return;
+  // V^T[b] = Wv . l[b]^T : A = weights (rows = channels), B = tokens
+  const int B = l.N, T = l.H * l.W, C = l.C;
+  const int Tp = ceil_div(T, 8) * 8;
+  const int PL = split_ ? 2 : 1;
+  const long long TpP = (long long)Tp * PL;
+  const size_t vt_bytes = (size_t)B * C * TpP * 2;
+  IgemmParams p;
+  std::memset(&p, 0, sizeof(p));
+  p.flags = bf16_ ? IG_BF16 : 0;
+  p.gridW = C; p.gridH = 1; p.TW = 128; p.TH = 1; p.tw_shift = 7;
+  p.Z1 = B; p.Z0 = 1;
+  p.b_z_z1 = 1;
+  p.nseg[0] = 1;
+  p.seg[0][0] = IgemmSeg{0, 0, 0, (uint16_t)(wv.ktot / 64)};
+  p.out = vT; p.outW = C; p.outH = 1;
+  p.out_pix_stride = TpP; p.out_row_stride = 0;
+  p.out_z1 = (long long)C * TpP;
+  p.out_sy = p.out_sx = 1;
+  p.Cout = T;
+  p.BN = choose_bn(T, 0);
+  const long long wrow = (long long)wv.ktot * PL;
+  check_cuda(make_tmap_a(&p.tmA[0], wv.w, wv.ktot, C, 1, 1, wrow, (long long)C * wrow, (long long)C * wrow,
+                         128, 1, bf16_), name + ": tmap Wv");
+  for (int i = 1; i < 4; ++i) p.tmA[i] = p.tmA[0];
+  check_cuda(make_tmap_b(&p.tmB, ptr(l), C, T, B, l.ps(), (long long)T * l.ps(), p.BN, bf16_), name + ": tmap l");
+  if (split_) {
+    check_cuda(make_tmap_a(&p.tmA[4], wv.w + wv.ktot, wv.ktot, C, 1, 1, wrow, (long long)C * wrow, (long long)C * wrow,
+                           128, 1, bf16_), name + ": tmap Wv lo");
+    for (int i = 5; i < 8; ++i) p.tmA[i] = p.tmA[4];
+    check_cuda(make_tmap_b(&p.tmB2, reinterpret_cast<const uint16_t*>(ptr(l)) + C, C, T, B, l.ps(), (long long)T * l.ps(), p.BN, bf16_),
+               name + ": tmap l lo");
+    set_passes(p);
+    p.out_lo = Tp;
+  }
+  finalize_or_throw(&p, name + ".to_vT");
+  push(name + ".to_vT", 1, 2.0 * B * (double)T * C * C, (double)vt_bytes + (double)l.bytes(),
+       [p](cudaStream_t s) { return igemm_launch(p, s); });
+  ops.back().kind = 1;
 }
 
 void Builder::gn_scale_shift(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps) {

@@ -4,11 +4,13 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <functional>
 #include <map>
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/genpercept_b200.h"
@@ -31,6 +33,22 @@ struct GpError : std::runtime_error {
   do {                                                                    \
     if (!(cond)) throw ::gp::GpError(GP_ERR_INVALID, std::string(msg));   \
   } while (0)
+
+constexpr float kLatentScale = 0.18215f;   // genpercept_pipeline.py:96
+
+inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// Output extent (Ho, Wo) of a convolution over an H x W input in ConvArgs::mode `mode`.
+inline std::pair<int, int> conv_out_dims(int mode, int H, int W) {
+  if (mode == 1) return {(H + 2 - 3) / 2 + 1, (W + 2 - 3) / 2 + 1};
+  if (mode == 2) return {(H + 1 - 3) / 2 + 1, (W + 1 - 3) / 2 + 1};
+  if (mode == 3) return {2 * H, 2 * W};
+  return {H, W};
+}
+
+// fp32 <-> 16-bit storage values (fp16, or bf16 when `bf16`), round to nearest
+uint16_t host_f2h(float f, bool bf16);
+float host_h2f(uint16_t u, bool bf16);
 
 struct HostT {
   std::vector<float> d;
@@ -127,6 +145,8 @@ class Builder {
   // generic batched GEMM pieces of attention; q/k/v views live inside `qk` / `l`
   void attention(const std::string& name, const T4& l, const PackedW& wqk, const PackedW& wv, const float* pv_bias,
                  int heads, const T4& out);
+  // V^T[b] = Wv . l[b]^T into vT: [B][C][Tp] with Tp = T rounded up to 8 (rows [hi Tp | lo Tp] in the high-precision mode)
+  void to_vT(const std::string& name, const T4& l, const PackedW& wv, void* vT);
   void attention_qkv(const std::string& name, const void* q, const void* k, long long qk_cstride, const void* vT, int B,
                      int T, int heads, int d, const float* pv_bias, const T4& out, long long qk_lo = 0);
   void gn(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps, bool silu,
@@ -165,6 +185,88 @@ class Builder {
   bool bf16_, measuring_, split_ = false;
   uint8_t* base_;
   Arena arena_;
+};
+
+// weights.cu: the checkpoint's host tensors and the device weights packed from them (constant folding + packing,
+// SURVEY.md App. C).  Every accessor packs and uploads on first use and returns the cached result afterwards, so one
+// measuring pass over a topology uploads exactly the weights that topology reaches.  The store owns every device
+// allocation it makes and frees them when it is destroyed.
+class WeightStore {
+ public:
+  explicit WeightStore(bool bf16 = false, bool split = false) : bf16(bf16), split(split) {}
+  ~WeightStore();
+  WeightStore(const WeightStore&) = delete;
+  WeightStore& operator=(const WeightStore&) = delete;
+
+  bool bf16;
+  bool split;                // cfg.precision == 1: (hi, lo) fp16 pairs everywhere (T4::planes, PackedW::planes)
+  std::unordered_map<std::string, HostT> host;
+  std::vector<float> text_embed;
+  int n_tokens = 0;
+  size_t weight_bytes = 0;
+  float* pq_dev = nullptr;   // vae.post_quant_conv: [16] weight + [4] bias, fp32 on the device
+  int cur_timestep = 0;
+
+  void put(const std::string& key, std::vector<int64_t> shape, const float* d);
+  template <class Tp>
+  Tp* upload(const std::vector<Tp>& v) {
+    void* d = device_alloc(std::max<size_t>(v.size() * sizeof(Tp), 16));
+    GP_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(Tp), cudaMemcpyHostToDevice));
+    weight_bytes += v.size() * sizeof(Tp);
+    return reinterpret_cast<Tp*>(d);
+  }
+  void* device_alloc(size_t bytes);   // freed with the store; not counted in weight_bytes
+
+  PackedW pack(const std::vector<std::vector<SegSpec>>& classes, int rows, const std::vector<float>& bias);
+  const PackedW& conv_w(const std::string& key, const std::vector<int>& srcC, const std::string& sc_key = "",
+                        const std::vector<int>& scC = {}, const std::vector<float>* extra_bias = nullptr,
+                        bool want_bias = true, const std::string& cache_suffix = "");
+  const PackedW& conv_up_w(const std::string& key);
+  const PackedW& mat_w(const std::string& cache_key, int rows, int K, const float* m, const std::vector<float>& bias);
+  const PackedW& lin_w(const std::string& key, bool bias = true);
+  const NormW& norm_w(const std::string& key);
+  const DirectW& direct_w(const std::string& key, int cin_used, const std::vector<float>* w_override = nullptr,
+                          const std::vector<float>* b_override = nullptr, int cout_override = 0);
+  const XattnW& xattn_w(const std::string& blk, int C, int heads);
+  struct XattnGen { const PackedW* A; const PackedW* B; int Kp; };
+  XattnGen xattn_general_w(const std::string& blk, int C, int heads);
+
+  // folded weights of the graph (weights.cu says what each one folds)
+  const PackedW& resnet_conv1(const std::string& p, int cin, bool temb_on);
+  const PackedW& self_attn_qk(const std::string& blk, int C, int heads);
+  const PackedW& geglu_w(const std::string& blk, int C);
+  const PackedW& vae_attn_qk(const std::string& a);
+  const float* vae_v_bias(const std::string& a);
+  const PackedW& encoder_conv_in();
+  const PackedW& encoder_tail();
+  const PackedW& unet_conv_out_plain();
+  const PackedW& unet_tail();
+  const PackedW& decoder_tail1();
+  int unet_in_channels();
+
+  void compute_temb(int timestep);
+  void set_timestep(int timestep);
+
+ private:
+  const HostT& T(const std::string& k) const;
+  bool has(const std::string& k) const { return host.count(k) != 0; }
+  void upload_post_quant();
+  std::vector<float> temb_for(int timestep) const;
+
+  std::vector<void*> dev_allocs;
+  std::unordered_map<std::string, PackedW> packed;
+  std::unordered_map<std::string, NormW> norms;
+  std::unordered_map<std::string, XattnW> xattns;
+  std::unordered_map<std::string, DirectW> directs;
+  std::unordered_map<std::string, float*> v_biases;
+  std::vector<float> temb;   // [1280] time embedding for the configured timestep
+  // Per-call fix_timesteps (genpercept_pipeline.py:405-408): the timestep only enters through
+  // conv1.bias + time_emb_proj(silu(emb(t))) of the 22 UNet ResNets, so changing it re-folds those biases in place
+  // (the device bias buffers keep their addresses: every plan and captured graph sees the new values).
+  struct TembLayer { std::vector<float> w, b, conv_bias; float* dev_bias = nullptr; int cout = 0; };
+  std::vector<TembLayer> temb_layers;
+  std::vector<float> te_w1, te_b1, te_w2, te_b2;
+  std::map<int, std::vector<std::vector<float>>> temb_cache;   // timestep -> folded bias per layer
 };
 
 // builder.cu: (BN, MT) of a stride-1 implicit-GEMM layer (default policy + the waves / L2-traffic model)
