@@ -1,7 +1,9 @@
 #!/usr/bin/env python
-"""Measurement behind the fused head-dim-512 attention of the VAE mid-block (csrc/fattn512.cu).
+"""Measurement behind the fused head-dim-512 attention of the VAE mid-block (csrc/fattn512.cu), and with
+--precision high behind the high-precision mode's memory-efficient attention (the split-precision instances of
+csrc/fattn.cu and csrc/fattn512.cu).
 
-  python bench_native.py [--iters N] [--skip-e2e]
+  python bench_native.py [--iters N] [--skip-e2e] [--precision default|high]
 
 Prints ONE JSON line:
 
@@ -14,6 +16,13 @@ Prints ONE JSON line:
   native       whole-engine inference (Engine.infer, the single_infer hot path) of one fp16 image at native photo
                sizes: ms per image (median of the timed calls, device-synchronised) and the plan's arena bytes.
   device       the card's name and power limit, read in the same run.
+
+With --precision high the line instead holds
+  attention    both high-precision paths (fused split-precision kernel; unfused QK^T -> softmax -> P V over (hi, lo)
+               planes) for d = 64 with 5 heads (the UNet's first level) and for d = 512 with one head, at the same B and
+               T: microseconds per call and TFLOP/s of the algorithmic 4 B heads T^2 d FLOPs (each takes three
+               tensor-core passes per product); null where the unfused path cannot run.
+  native       the same native sizes through the high-precision engine with memory-efficient attention on.
 
 Weights and inputs are seeded synthetic data; nothing is written to the tree.
 """
@@ -51,6 +60,29 @@ def device_info():
     return info
 
 
+def attention_sweep_high(iters):
+    from genpercept_b200 import engine as E
+    rows = []
+    for heads, d in ((5, 64), (1, 512)):
+        for B in BATCHES:
+            for T in TOKENS:
+                tp = (T + 7) // 8 * 8
+                unfused_runs = T % 8 != 0 or T <= SOFTMAX_ROWS_MAX_T
+                row = {"heads": heads, "d": d, "B": B, "T": T, "s_bytes": B * heads * T * 2 * tp * 2}
+                for path, fused in (("fused", True), ("unfused", False)):
+                    if not fused and not unfused_runs:
+                        row[path] = None
+                        continue
+                    us, fl = E.bench_attention_high(B, T, heads, d, fused, iters)
+                    row[path] = {"usec": round(us, 1), "tflops": round(fl / us * 1e-6, 1)}
+                    torch.cuda.empty_cache()
+                if row["unfused"]:
+                    row["fused_over_unfused"] = round(row["fused"]["usec"] / row["unfused"]["usec"], 3)
+                rows.append(row)
+                print(json.dumps(row), file=sys.stderr, flush=True)
+    return rows
+
+
 def attention_sweep(iters):
     from genpercept_b200 import engine as E
     rows = []
@@ -75,12 +107,15 @@ def attention_sweep(iters):
     return rows
 
 
-def native_sweep(reps):
+def native_sweep(reps, precision="default"):
     from genpercept_b200 import weights as W
     from genpercept_b200.engine import Engine
     state = W.synth_state(1234, with_dpt=False)
     te = torch.from_numpy(np.load(os.path.join(ROOT, "tests", "golden", "empty_text_embed_2x1024.npy")).astype(np.float32))[None]
-    e = Engine(dtype=torch.float16, readout="vae")
+    high = precision == "high"
+    if high:   # the high-precision arenas (~30 GB at these sizes) do not fit the default four cached plans
+        os.environ["GP_MAX_PLANS"] = "1"
+    e = Engine(dtype=torch.float16, readout="vae", precision=precision, memory_efficient_attention=high)
     e.load_state("unet", state["unet"])
     e.load_state("vae", state["vae"])
     e.set_text_embed(te)
@@ -102,7 +137,7 @@ def native_sweep(reps):
             names = [op["name"] for op in e.profile_ops()]
             r = {"H": H, "W": W_, "T_mid": (H // 8) * (W_ // 8), "ms_per_image": round(statistics.median(ts), 1),
                  "ms_all": [round(t, 1) for t in ts], "arena_bytes": info["arena_bytes"],
-                 "fused_attention_ops": sum(n.endswith(".fattn512") for n in names),
+                 "fused_attention_ops": sum(n.endswith((".fattn512", ".fattn") if high else ".fattn512") for n in names),
                  "finite": bool(torch.isfinite(out).all().item())}
             res.append(r)
             print(json.dumps(r), file=sys.stderr, flush=True)
@@ -116,14 +151,19 @@ def main():
     ap.add_argument("--iters", type=int, default=5, help="timed calls per attention configuration")
     ap.add_argument("--reps", type=int, default=3, help="timed images per native size")
     ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--precision", choices=("default", "high"), default="default")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_native.py needs a CUDA device (H100)")
     dev = device_info()
-    line = {"device": dev, "peak_fp16_dense_tflops_datasheet": PEAK_FP16_DENSE_TFLOPS,
-            "attention": attention_sweep(a.iters)}
+    if a.precision == "high":
+        line = {"device": dev, "precision": "high", "peak_fp16_dense_tflops_datasheet": PEAK_FP16_DENSE_TFLOPS,
+                "attention": attention_sweep_high(a.iters)}
+    else:
+        line = {"device": dev, "peak_fp16_dense_tflops_datasheet": PEAK_FP16_DENSE_TFLOPS,
+                "attention": attention_sweep(a.iters)}
     if not a.skip_e2e:
-        line["native"] = native_sweep(a.reps)
+        line["native"] = native_sweep(a.reps, a.precision)
     print(json.dumps(line))
 
 

@@ -498,6 +498,21 @@ static void set_passes(IgemmParams& p) {
   p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = 1;
 }
 
+// The lo-plane tensor maps of a fused attention kernel in the high-precision mode (FattnParams / Fattn512Params)
+template <class P>
+static void set_split_maps(P& p, const void* q, const void* k, const void* vT, int C, int T, int B, long long cs,
+                           long long qk_lo, int Tp, int q_box, int out_lo, const std::string& name) {
+  const uint16_t* ql = reinterpret_cast<const uint16_t*>(q) + qk_lo;
+  const uint16_t* kl = reinterpret_cast<const uint16_t*>(k) + qk_lo;
+  const uint16_t* vl = reinterpret_cast<const uint16_t*>(vT) + Tp;
+  const long long TpP = 2LL * Tp;
+  check_cuda(make_tmap_b(&p.tmQl, ql, C, T, B, cs, (long long)T * cs, q_box, false), name + ": tmap Q lo");
+  check_cuda(make_tmap_b(&p.tmKl, kl, C, T, B, cs, (long long)T * cs, q_box, false), name + ": tmap K lo");
+  check_cuda(make_tmap_b(&p.tmVl, vl, T, C, B, TpP, (long long)C * TpP, 64, false), name + ": tmap Vt lo");
+  p.split = 1;
+  p.out_lo = out_lo;
+}
+
 void Builder::attention_qkv(const std::string& name, const void* q, const void* k, long long cs, const void* vT, int B,
                             int T, int heads, int d, const float* pv_bias, const T4& out, long long qk_lo) {
   // High-precision mode: q / k carry their lo planes `qk_lo` elements further (same pixel stride cs), V^T rows are
@@ -506,20 +521,24 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
   const int C = heads * d;
   const int PL = split_ ? 2 : 1;
   const long long TpP = (long long)Tp * PL;   // physical row pitch of S and V^T
-  if (d == 64 && !split_) {   // fused wgmma flash-attention kernel (S and P stay on chip)
+  // The high-precision mode takes the fused kernels only when memory-efficient attention is switched on; by default
+  // its plans store S.
+  const bool split_fused = split_ && mem_efficient_attn;
+  if (d == 64 && (!split_ || split_fused)) {   // fused wgmma flash-attention kernel (S and P stay on chip)
     if (measuring_) return;
     FattnParams p;
     std::memset(&p, 0, sizeof(p));
     p.out = ptr(out);
-    p.out_b_stride = (long long)T * C;
-    p.out_row_stride = C;
+    p.out_b_stride = (long long)T * out.ps();
+    p.out_row_stride = (int)out.ps();
     p.T = T; p.heads = heads; p.B = B; p.q_tiles = ceil_div(T, 128);
     p.scale_log2e = 1.4426950408889634f;
     p.bf16 = bf16_ ? 1 : 0;
     check_cuda(make_tmap_b(&p.tmQ, q, C, T, B, cs, (long long)T * cs, 128, bf16_), name + ": tmap Q");
     check_cuda(make_tmap_b(&p.tmK, k, C, T, B, cs, (long long)T * cs, 128, bf16_), name + ": tmap K");
-    check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, Tp, (long long)C * Tp, 64, bf16_), name + ": tmap Vt");
-    push(name + ".fattn", 1, 4.0 * B * heads * (double)T * T * d, 4.0 * B * T * C * 2,
+    check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, TpP, (long long)C * TpP, 64, bf16_), name + ": tmap Vt");
+    if (split_) set_split_maps(p, q, k, vT, C, T, B, cs, qk_lo, Tp, 128, out.C, name);
+    push(name + ".fattn", 1, 4.0 * B * heads * (double)T * T * d, 4.0 * B * T * C * 2 * PL,
          [p](cudaStream_t s) { return fattn_launch(p, s); });
     ops.back().kind = 2;
     return;
@@ -527,8 +546,9 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
   const size_t s_bytes = (size_t)B * heads * T * TpP * 2;
   // the unfused path's softmax_rows cannot take rows past kSoftmaxRowsMaxT keys when T is a multiple of 8
   const bool unfused_runs = T % 8 != 0 || T <= kSoftmaxRowsMaxT;
-  const bool fused512 = d == 512 && heads == 1 && !split_ &&
-                        (attn512_path >= 0 ? attn512_path == 1 : s_bytes > kFusedAttnMinBytes || !unfused_runs);
+  const bool fused512 = d == 512 && heads == 1 &&
+                        (split_ ? split_fused
+                                : attn512_path >= 0 ? attn512_path == 1 : s_bytes > kFusedAttnMinBytes || !unfused_runs);
   if (fused512) {   // fused d = 512 kernel: no score matrix in the arena
     if (measuring_) return;
     Fattn512Params p;
@@ -542,12 +562,14 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
     p.bf16 = bf16_ ? 1 : 0;
     check_cuda(make_tmap_b(&p.tmQ, q, C, T, B, cs, (long long)T * cs, 64, bf16_), name + ": tmap Q");
     check_cuda(make_tmap_b(&p.tmK, k, C, T, B, cs, (long long)T * cs, 64, bf16_), name + ": tmap K");
-    check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, Tp, (long long)C * Tp, 64, bf16_), name + ": tmap Vt");
-    push(name + ".fattn512", 1, 4.0 * B * (double)T * T * d, 4.0 * B * T * C * 2,
+    check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, TpP, (long long)C * TpP, 64, bf16_), name + ": tmap Vt");
+    if (split_) set_split_maps(p, q, k, vT, C, T, B, cs, qk_lo, Tp, 64, out.C, name);
+    push(name + ".fattn512", 1, 4.0 * B * (double)T * T * d, 4.0 * B * T * C * 2 * PL,
          [p](cudaStream_t s) { return fattn512_launch(p, s); });
     ops.back().kind = 2;
     return;
   }
+  if (!unfused_runs && long_softmax.empty()) long_softmax = name;
   const size_t s_off = arena_.alloc(s_bytes);
   if (!measuring_) {
     void* S = raw_ptr(s_off);

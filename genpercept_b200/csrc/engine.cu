@@ -56,6 +56,16 @@ struct gp_engine {
   uint64_t use_clock = 0;
   std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>> plans;
   Plan* cur = nullptr;
+  bool mem_efficient_attn = false;   // gp_set_memory_efficient_attention: fused attention in the high-precision mode
+
+  // Synchronises, then destroys a cached plan's graph execs and frees its arena.
+  void drop_plan(std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>>::iterator it) {
+    GP_CUDA(cudaDeviceSynchronize());
+    for (auto& g : it->second->graphs) cudaGraphExecDestroy(g.second);
+    if (it->second->arena) cudaFree(it->second->arena);
+    if (cur == it->second.get()) cur = nullptr;
+    plans.erase(it);
+  }
 
   // ------------------------------------------------------------------ graph pieces
   // 3x3 conv whose input is an NHWC8 tensor with `cin` (4 or 8) real channels: one 64-wide K chunk
@@ -675,13 +685,10 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
       auto victim = e->plans.begin();
       for (auto jt = e->plans.begin(); jt != e->plans.end(); ++jt)
         if (jt->second->last_used < victim->second->last_used) victim = jt;
-      GP_CUDA(cudaDeviceSynchronize());
-      for (auto& g : victim->second->graphs) cudaGraphExecDestroy(g.second);
-      if (victim->second->arena) cudaFree(victim->second->arena);
-      if (e->cur == victim->second.get()) e->cur = nullptr;
-      e->plans.erase(victim);
+      e->drop_plan(victim);
     }
     Builder m(e->ws.bf16, true, nullptr, e->ws.split);
+    m.mem_efficient_attn = e->mem_efficient_attn;
     e->build(m, nullptr, B, H, W);
     std::unique_ptr<Plan> p(new Plan());
     p->B = B; p->H = H; p->W = W;
@@ -696,8 +703,18 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
                                         std::to_string(p->arena_bytes) + " bytes, more than the device can allocate");
     }
     GP_CUDA(ae);
+    if (!m.long_softmax.empty()) {
+      // The arena fits, but the unfused softmax of this attention cannot run: fail here, not with a CUDA error at
+      // inference, and leave the engine usable.
+      cudaFree(p->arena);
+      throw GpError(GP_ERR_INVALID, "gp_plan: batch " + std::to_string(B) + " at " + std::to_string(H) + "x" +
+                                        std::to_string(W) + ": " + m.long_softmax + " has rows past " +
+                                        std::to_string(kSoftmaxRowsMaxT) + " keys, more than the unfused softmax takes; "
+                                        "enable memory-efficient attention (gp_set_memory_efficient_attention)");
+    }
     GP_CUDA(cudaMemset(p->arena, 0, p->arena_bytes));
     Builder b(e->ws.bf16, false, p->arena, e->ws.split);
+    b.mem_efficient_attn = e->mem_efficient_attn;
     e->build(b, p.get(), B, H, W);
     if (b.arena_bytes() != p->arena_bytes) throw GpError(GP_ERR_STATE, "planner passes disagree on arena size");
     p->ops = std::move(b.ops);
@@ -713,6 +730,16 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
 }
 
 int gp_plan_count(gp_engine* e) { return e ? (int)e->plans.size() : 0; }
+
+gp_status gp_set_memory_efficient_attention(gp_engine* e, int enable) {
+  return guarded(e, [&]() {
+    const bool on = enable != 0;
+    if (on == e->mem_efficient_attn) return;
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    while (!e->plans.empty()) e->drop_plan(e->plans.begin());
+    e->mem_efficient_attn = on;
+  });
+}
 
 gp_status gp_tile_shape(int cout, int cin, int ks, int images, int h, int w, int tokens_mode, int num_sms, int* bn, int* mt) {
   if (!bn || !mt || cout < 1 || cin < 1 || ks < 1 || images < 1 || h < 1 || w < 1 || num_sms < 1) return GP_ERR_INVALID;

@@ -178,6 +178,12 @@ class Builder {
   // Single-head d = 512 attention path: -1 chooses by the size of the score matrix (kFusedAttnMinBytes, builder.cu);
   // 0 forces the unfused path, 1 the fused kernel.  Only gp_bench_attention sets it, to time both paths at one shape.
   int attn512_path = -1;
+  // High-precision mode: run every d = 64 and single-head d = 512 attention through the fused kernels, so no score matrix
+  // is stored (gp_set_memory_efficient_attention).  The 16-bit modes ignore it.
+  bool mem_efficient_attn = false;
+  // Set when an unfused attention was planned whose softmax_rows cannot run (rows past kSoftmaxRowsMaxT keys with T a
+  // multiple of 8): the name of the first such op.
+  std::string long_softmax;
 
  private:
   void push(const std::string& name, int launches, double flops, double bytes,

@@ -11,10 +11,16 @@
 //                   registers whenever the running maximum grows.
 //
 // S and P never touch shared memory or HBM.
+//
+// SPLIT (the high-precision mode): every operand is an fp16 (hi, lo) pair.  The Q tile and each ring stage carry both
+// planes (3 stages of K hi | K lo | V^T hi | V^T lo); S = Qh Kh^T + Ql Kh^T + Qh Kl^T in fp32, P is split in registers
+// into ph = f16(p), pl = f16(p - ph), O += Ph Vh + Pl Vh + Ph Vl, and O is stored as its (hi, lo) pair.
 #include "fattn.h"
 
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+
+#include <utility>
 
 #include "launch.h"
 #include "ptx.cuh"
@@ -23,11 +29,14 @@ namespace gp {
 namespace {
 
 constexpr int kThreads = 288;                  // two consumer warpgroups + the producer warp
-constexpr int kStages = 4;
-constexpr int kQBytes = 128 * 64 * 2;          // 16 KiB
-constexpr int kKBytes = 128 * 64 * 2;          // 16 KiB
-constexpr int kVBytes = 64 * 128 * 2;          // 16 KiB (two 64-key sub-tiles of 8 KiB)
-constexpr int kSmemBytes = kQBytes + kStages * (kKBytes + kVBytes) + 256 + 1024;
+constexpr int kQBytes = 128 * 64 * 2;          // 16 KiB per plane
+constexpr int kKBytes = 128 * 64 * 2;          // 16 KiB per plane
+constexpr int kVBytes = 64 * 128 * 2;          // 16 KiB per plane (two 64-key sub-tiles of 8 KiB)
+template <bool SPLIT> constexpr int kPlanesOf = SPLIT ? 2 : 1;
+template <bool SPLIT> constexpr int kStagesOf = SPLIT ? 3 : 4;
+template <bool SPLIT>
+constexpr int kSmemBytes = kPlanesOf<SPLIT> * (kQBytes + kStagesOf<SPLIT> * (kKBytes + kVBytes)) + 256 + 1024;
+static_assert(kSmemBytes<true> <= 227 * 1024, "shared memory of one CTA");
 
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -44,6 +53,14 @@ __device__ __forceinline__ uint32_t pack16(float a, float b) {
     return *reinterpret_cast<uint32_t*>(&h);
   }
 }
+// fp32 pair -> its fp16 (hi, lo) pairs: hi = f16(x), lo = f16(x - hi)
+__device__ __forceinline__ void split16(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const float2 f = __half22float2(h);
+  const __half2 l = __floats2half2_rn(a - f.x, b - f.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -53,14 +70,16 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <bool BF16>
+template <bool BF16, bool SPLIT>
 __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constant__ FattnParams p) {
+  static_assert(!(BF16 && SPLIT), "the high-precision mode uses fp16 pairs");
+  constexpr int PL = kPlanesOf<SPLIT>, kStages = kStagesOf<SPLIT>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                               // [16 KiB]
-  uint8_t* sK = sQ + kQBytes;                       // [stage][16 KiB]
-  uint8_t* sV = sK + kStages * kKBytes;             // [stage][16 KiB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kStages * kVBytes);
+  uint8_t* sQ = smem;                               // [plane][16 KiB]
+  uint8_t* sK = sQ + PL * kQBytes;                  // [stage][plane][16 KiB]
+  uint8_t* sV = sK + kStages * PL * kKBytes;        // [stage][plane][16 KiB]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kStages * PL * kVBytes);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;                     // [kStages]
   uint64_t* kv_empty = kv_full + kStages;           // [kStages]  one arrival per consumer warp
@@ -76,6 +95,11 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);
+    if constexpr (SPLIT) {
+      tma_prefetch_desc(&p.tmQl);
+      tma_prefetch_desc(&p.tmKl);
+      tma_prefetch_desc(&p.tmVl);
+    }
     mbar_init(q_full, 1);
     for (int i = 0; i < kStages; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 8); }
     fence_barrier_init();
@@ -86,17 +110,25 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
     // ------------------------------------------------------------------ TMA producer (whole warp waits, one lane issues)
     const bool leader = elect_one();
     if (leader) {
-      mbar_expect_tx(q_full, (uint32_t)kQBytes);
+      mbar_expect_tx(q_full, (uint32_t)(PL * kQBytes));
       tma_load_3d(sQ, &p.tmQ, q_full, head * 64, qt * 128, b);
+      if constexpr (SPLIT) tma_load_3d(sQ + kQBytes, &p.tmQl, q_full, head * 64, qt * 128, b);
     }
     for (int j = 0; j < nblk; ++j) {
       const int st = j % kStages;
       mbar_wait(&kv_empty[st], ((j / kStages) & 1) ^ 1, 10);
       if (leader) {
-        mbar_expect_tx(&kv_full[st], kKBytes + kVBytes);
-        tma_load_3d(sK + st * kKBytes, &p.tmK, &kv_full[st], head * 64, j * 128, b);
-        tma_load_3d(sV + st * kVBytes, &p.tmV, &kv_full[st], j * 128, head * 64, b);
-        tma_load_3d(sV + st * kVBytes + 8192, &p.tmV, &kv_full[st], j * 128 + 64, head * 64, b);
+        mbar_expect_tx(&kv_full[st], PL * (kKBytes + kVBytes));
+        uint8_t* k_st = sK + st * PL * kKBytes;
+        uint8_t* v_st = sV + st * PL * kVBytes;
+        tma_load_3d(k_st, &p.tmK, &kv_full[st], head * 64, j * 128, b);
+        tma_load_3d(v_st, &p.tmV, &kv_full[st], j * 128, head * 64, b);
+        tma_load_3d(v_st + 8192, &p.tmV, &kv_full[st], j * 128 + 64, head * 64, b);
+        if constexpr (SPLIT) {
+          tma_load_3d(k_st + kKBytes, &p.tmKl, &kv_full[st], head * 64, j * 128, b);
+          tma_load_3d(v_st + kVBytes, &p.tmVl, &kv_full[st], j * 128, head * 64, b);
+          tma_load_3d(v_st + kVBytes + 8192, &p.tmVl, &kv_full[st], j * 128 + 64, head * 64, b);
+        }
       }
       __syncwarp();
     }
@@ -114,11 +146,19 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
       const int st = j % kStages;
       mbar_wait(&kv_full[st], (j / kStages) & 1, 11);
       float s[64];
-      const uint64_t k_desc = make_sw128_kmajor_desc(smem_u32(sK + st * kKBytes));
+      const uint64_t k_desc = make_sw128_kmajor_desc(smem_u32(sK + st * PL * kKBytes));
       reg_fence(s);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) wgmma_ss_n128<BF16>(s, q_desc + 2 * k, k_desc + 2 * k, k ? 1u : 0u);
+      if constexpr (SPLIT) {   // + Ql Kh^T + Qh Kl^T  (descriptor addresses are in 16-byte units)
+        constexpr uint64_t kQlo = kQBytes >> 4, kKlo = kKBytes >> 4;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_ss_n128<false>(s, q_desc + kQlo + 2 * k, k_desc + 2 * k, 1u);
+          wgmma_ss_n128<false>(s, q_desc + 2 * k, k_desc + kKlo + 2 * k, 1u);
+        }
+      }
       wgmma_commit();
       wgmma_wait<0>();
       reg_fence(s);
@@ -159,15 +199,24 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
         o[4 * i + 2] *= a1; o[4 * i + 3] *= a1;
       }
       // P as the register A operand: k step kk (keys 16 kk ..) = accumulator columns of n blocks 2 kk, 2 kk + 1
-      const uint32_t v_base = smem_u32(sV + st * kVBytes);
+      const uint32_t v_base = smem_u32(sV + st * PL * kVBytes);
       reg_fence(o);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) {
-        const uint32_t a[4] = {pack16<BF16>(s[8 * kk], s[8 * kk + 1]), pack16<BF16>(s[8 * kk + 2], s[8 * kk + 3]),
-                               pack16<BF16>(s[8 * kk + 4], s[8 * kk + 5]), pack16<BF16>(s[8 * kk + 6], s[8 * kk + 7])};
         const uint64_t v_desc = make_sw128_kmajor_desc(v_base + (kk >> 2) * 8192) + 2 * (kk & 3);
-        wgmma_rs_n64<BF16>(o, a, v_desc, 1u);
+        if constexpr (SPLIT) {   // Ph Vh + Pl Vh + Ph Vl
+          uint32_t ah[4], al[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) split16(s[8 * kk + 2 * e], s[8 * kk + 2 * e + 1], ah[e], al[e]);
+          wgmma_rs_n64<false>(o, ah, v_desc, 1u);
+          wgmma_rs_n64<false>(o, al, v_desc, 1u);
+          wgmma_rs_n64<false>(o, ah, v_desc + (kVBytes >> 4), 1u);
+        } else {
+          const uint32_t a[4] = {pack16<BF16>(s[8 * kk], s[8 * kk + 1]), pack16<BF16>(s[8 * kk + 2], s[8 * kk + 3]),
+                                 pack16<BF16>(s[8 * kk + 4], s[8 * kk + 5]), pack16<BF16>(s[8 * kk + 6], s[8 * kk + 7])};
+          wgmma_rs_n64<BF16>(o, a, v_desc, 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -186,8 +235,16 @@ __global__ void __launch_bounds__(kThreads, 1) fattn_kernel(const __grid_constan
       const float inv = hh ? inv1 : inv0;
       uint16_t* op = ob + (long long)row * p.out_row_stride;
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        *reinterpret_cast<uint32_t*>(op + 8 * i) = pack16<BF16>(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+      for (int i = 0; i < 8; ++i) {
+        if constexpr (SPLIT) {
+          uint32_t hi, lo;
+          split16(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv, hi, lo);
+          *reinterpret_cast<uint32_t*>(op + 8 * i) = hi;
+          *reinterpret_cast<uint32_t*>(op + p.out_lo + 8 * i) = lo;
+        } else {
+          *reinterpret_cast<uint32_t*>(op + 8 * i) = pack16<BF16>(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+        }
+      }
     }
   }
 }
@@ -200,17 +257,20 @@ cudaError_t fattn_launch(const FattnParams& p, cudaStream_t stream) {
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   if (!attr_dev[dev]) {      // function attributes are per device
-    const void* fns[2] = {(const void*)fattn_kernel<false>, (const void*)fattn_kernel<true>};
-    for (const void* f : fns) {
-      cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    const std::pair<const void*, int> fns[3] = {{(const void*)fattn_kernel<false, false>, kSmemBytes<false>},
+                                                {(const void*)fattn_kernel<true, false>, kSmemBytes<false>},
+                                                {(const void*)fattn_kernel<false, true>, kSmemBytes<true>}};
+    for (auto [f, bytes] : fns) {
+      cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
       if (e != cudaSuccess) return e;
     }
     attr_dev[dev] = true;
   }
   const int grid = p.B * p.heads * p.q_tiles;
   if (grid <= 0) return cudaSuccess;
-  if (p.bf16) launch(fattn_kernel<true>, grid, kThreads, kSmemBytes, stream, p);
-  else launch(fattn_kernel<false>, grid, kThreads, kSmemBytes, stream, p);
+  if (p.split) launch(fattn_kernel<false, true>, grid, kThreads, kSmemBytes<true>, stream, p);
+  else if (p.bf16) launch(fattn_kernel<true, false>, grid, kThreads, kSmemBytes<false>, stream, p);
+  else launch(fattn_kernel<false, false>, grid, kThreads, kSmemBytes<false>, stream, p);
   return cudaGetLastError();
 }
 

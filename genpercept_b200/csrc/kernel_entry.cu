@@ -33,9 +33,11 @@ void run_all(Builder& b, cudaStream_t s) {
 // arena's base.
 template <class F>
 Builder build_and_run(WeightStore& ws, cudaStream_t s, F emit) {
-  Builder m(ws.bf16, true, nullptr);
+  Builder m(ws.bf16, true, nullptr, ws.split);
   emit(m);
-  Builder b(ws.bf16, false, reinterpret_cast<uint8_t*>(ws.device_alloc(m.arena_bytes() + 1024)));
+  GP_REQUIRE(m.long_softmax.empty(), m.long_softmax + ": rows past " + std::to_string(kSoftmaxRowsMaxT) +
+                                         " keys, more than the unfused softmax takes");
+  Builder b(ws.bf16, false, reinterpret_cast<uint8_t*>(ws.device_alloc(m.arena_bytes() + 1024)), ws.split);
   emit(b);
   run_all(b, s);
   GP_CUDA(cudaStreamSynchronize(s));
@@ -201,6 +203,28 @@ gp_status gp_attention(int dtype, const void* q, const void* k, const void* v, i
   });
 }
 
+gp_status gp_attention_high(const void* qk, const void* v, int B, int T, int heads, int d, int fused, void* o, void* stream) {
+  return guarded_free([&]() {
+    GP_REQUIRE(qk && v && o && B >= 1 && T >= 1 && (d == 64 || (d == 512 && heads == 1)),
+               "gp_attention_high: bad arguments (d = 64, or d = 512 with one head)");
+    // V^T is the engine's swapped-operand GEMM with identity weights (hi 1, lo 0), which reproduces v's (hi, lo) pairs
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    WeightStore ws(false, true);
+    const int C = heads * d;
+    const int Tp = ceil_div(T, 8) * 8;
+    std::vector<float> eye((size_t)C * C, 0.f);
+    for (int i = 0; i < C; ++i) eye[(size_t)i * C + i] = 1.f;
+    const PackedW& wv = ws.mat_w("eye", C, C, eye.data(), {});
+    void* vT = ws.device_alloc((size_t)B * C * 2 * Tp * 2);
+    build_and_run(ws, s, [&](Builder& b) {
+      b.mem_efficient_attn = fused != 0;
+      b.to_vT("v", b.external(v, B, 1, T, C), wv, vT);
+      const uint16_t* q = reinterpret_cast<const uint16_t*>(qk);
+      b.attention_qkv("attn", q, q + C, 4LL * C, vT, B, T, heads, d, nullptr, b.external(o, B, 1, T, C), 2LL * C);
+    });
+  });
+}
+
 gp_status gp_ensemble_reduce(const float* pred_dev, int B, int H, int W, const float* scale_host, const float* shift_host,
                              int median, int normalise, float* out_dev, void* stream) {
   return guarded_free([&]() {
@@ -291,6 +315,44 @@ gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, doub
     const double us = time_ops(b, iters);
     if (usec) *usec = us;
     if (flops) *flops = 4.0 * B * (double)T * T * C;
+  });
+}
+
+gp_status gp_bench_attention_high(int B, int T, int heads, int d, int fused, int iters, double* usec, double* flops) {
+  return guarded_free([&]() {
+    GP_REQUIRE(B >= 1 && T >= 1 && iters >= 1 && (d == 64 || (d == 512 && heads == 1)),
+               "gp_bench_attention_high: bad arguments (d = 64, or d = 512 with one head)");
+    WeightStore ws(false, true);
+    const int C = heads * d;
+    const int Tp = ceil_div(T, 8) * 8;
+    // the engine's operands: [q hi | k hi | q lo | k lo] per token, V^T [B][C][hi Tp | lo Tp], out [B][T][hi C | lo C]
+    const size_t qk_n = (size_t)B * T * 4 * C, vt_n = (size_t)B * C * 2 * Tp, o_n = (size_t)B * T * 2 * C;
+    void* qk = ws.device_alloc(qk_n * 2);
+    void* vT = ws.device_alloc(vt_n * 2);
+    void* o = ws.device_alloc(o_n * 2);
+    // small pseudo-random operands (scores of order one), lo planes included, so the tensor cores switch as on real data
+    {
+      std::vector<uint16_t> pat((size_t)1 << 20);
+      uint32_t x = 12345u;
+      for (auto& v : pat) {
+        x = x * 1664525u + 1013904223u;
+        const float f = ((int)(x >> 9) - (1 << 22)) * (0.3f / (1 << 22));
+        v = host_f2h(f, false);
+      }
+      for (auto [buf, n] : {std::make_pair(qk, qk_n), std::make_pair(vT, vt_n)})
+        for (size_t i = 0; i < n; i += pat.size())
+          GP_CUDA(cudaMemcpy(reinterpret_cast<uint16_t*>(buf) + i, pat.data(), std::min(pat.size(), n - i) * 2,
+                             cudaMemcpyHostToDevice));
+    }
+    // one warm-up launch, synchronised
+    Builder b = build_and_run(ws, 0, [&](Builder& bb) {
+      bb.mem_efficient_attn = fused != 0;
+      const uint16_t* q = reinterpret_cast<const uint16_t*>(qk);
+      bb.attention_qkv("attn", q, q + C, 4LL * C, vT, B, T, heads, d, nullptr, bb.external(o, B, 1, T, C), 2LL * C);
+    });
+    const double us = time_ops(b, iters);
+    if (usec) *usec = us;
+    if (flops) *flops = 4.0 * B * heads * (double)T * T * d;
   });
 }
 

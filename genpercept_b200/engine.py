@@ -56,6 +56,7 @@ def lib():
                                  c_int, c_int, c_void_p]
     L.gp_ensemble_reduce.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
     L.gp_plan_count.argtypes = [c_void_p]
+    L.gp_set_memory_efficient_attention.argtypes = [c_void_p, c_int]
     L.gp_tile_shape.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]
     L.gp_tensor_shape.argtypes = [c_void_p, c_char_p, POINTER(c_int64)]
     L.gp_read_tensor.argtypes = [c_void_p, c_char_p, c_void_p, c_size_t]
@@ -79,6 +80,8 @@ def lib():
     L.gp_bench_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_double),
                                 POINTER(c_double)]
     L.gp_bench_attention.argtypes = [c_int, c_int, c_int, c_int, c_int, POINTER(c_double), POINTER(c_double)]
+    L.gp_attention_high.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    L.gp_bench_attention_high.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_double), POINTER(c_double)]
     L.gp_resize_aa.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
                                c_int, c_void_p]
     L.gp_colorize.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_int,
@@ -105,7 +108,7 @@ class Engine:
     """One engine per (process, GPU).  Mirrors the C-ABI one to one."""
 
     def __init__(self, dtype=torch.float16, readout="vae", timestep=1, device=0, cuda_graph="auto",
-                 precision="default", arch="genpercept"):
+                 precision="default", arch="genpercept", memory_efficient_attention=False):
         if not torch.cuda.is_available():
             raise RuntimeError("genpercept_b200 needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.L = lib()
@@ -123,6 +126,18 @@ class Engine:
             raise RuntimeError(f"gp_create failed: {_STATUS.get(st, st)} (no sm_90a device?)")
         self.plan_shape = None
         self.out_hw = None
+        self.memory_efficient_attention = False
+        if memory_efficient_attention:
+            self.set_memory_efficient_attention(True)
+
+    def set_memory_efficient_attention(self, flag):
+        """High-precision mode: run every attention fused, storing no T x T score matrix (gp_set_memory_efficient_attention).
+        The 16-bit modes ignore it.  A change drops the cached plans; the next call plans again."""
+        self._ck(self.L.gp_set_memory_efficient_attention(self.h, 1 if flag else 0), "gp_set_memory_efficient_attention")
+        if bool(flag) != self.memory_efficient_attention:
+            self.plan_shape = None
+            self.out_hw = None
+        self.memory_efficient_attention = bool(flag)
 
     def close(self):
         if getattr(self, "h", None):
@@ -369,6 +384,29 @@ def attention(q, k, v, heads, scale):
     return o
 
 
+def split_hi_lo(x):
+    """fp32 -> its fp16 (hi, lo) pair, value = hi + lo: the high-precision mode's operand format."""
+    x = x.float()
+    hi = x.half()
+    return hi, (x - hi.float()).half()
+
+
+def attention_high(q, k, v, heads, scale, fused):
+    """High-precision attention (gp_attention_high): q, k, v cuda fp32 [B,T,heads*d] -> fp32 o = hi + lo.  scale * q
+    is split into its (hi, lo) pair, as are k and v; `fused` picks the fused split-precision kernel or the unfused path."""
+    B, T, C = q.shape
+    qh, ql = split_hi_lo(q * scale)
+    kh, kl = split_hi_lo(k)
+    vh, vl = split_hi_lo(v)
+    qk = torch.cat([qh, kh, ql, kl], dim=-1).contiguous()
+    vv = torch.cat([vh, vl], dim=-1).contiguous()
+    o = torch.zeros((B, T, 2 * C), dtype=torch.float16, device=q.device)
+    st = lib().gp_attention_high(c_void_p(qk.data_ptr()), c_void_p(vv.data_ptr()), B, T, heads, C // heads, 1 if fused else 0,
+                                 c_void_p(o.data_ptr()), _stream_ptr(q.device))
+    _check_free(st, "gp_attention_high")
+    return o[..., :C].float() + o[..., C:].float()
+
+
 def bilinear_up2x(x_nhwc):
     N, H, W, C = x_nhwc.shape
     y = torch.empty((N, 2 * H, 2 * W, C), dtype=x_nhwc.dtype, device=x_nhwc.device)
@@ -452,4 +490,13 @@ def bench_attention(dtype, B, T, fused, iters=10):
     us, fl = c_double(), c_double()
     st = lib().gp_bench_attention(_gp_dtype(dtype), B, T, 1 if fused else 0, iters, byref(us), byref(fl))
     _check_free(st, "gp_bench_attention")
+    return us.value, fl.value
+
+
+def bench_attention_high(B, T, heads, d, fused, iters=10):
+    """Time the fused or the unfused high-precision attention (d = 64 with `heads` heads, or d = 512 with one) at B x T
+    tokens.  Returns (microseconds per call, FLOPs per call)."""
+    us, fl = c_double(), c_double()
+    st = lib().gp_bench_attention_high(B, T, heads, d, 1 if fused else 0, iters, byref(us), byref(fl))
+    _check_free(st, "gp_bench_attention_high")
     return us.value, fl.value

@@ -173,8 +173,15 @@ class GenPerceptPipeline:
     def to(self, *a, **k):
         return self
 
-    def enable_xformers_memory_efficient_attention(self, *a, **k):   # run.py:382-385 calls this in a try
-        return None
+    def enable_xformers_memory_efficient_attention(self, *a, **k):   # run.py:382-385, infer.py:400-403
+        """Memory-efficient attention: in the high-precision mode (torch_dtype=float32) every attention runs fused and
+        stores no T x T score matrix, so native-resolution photos fit.  The 16-bit modes already bound it.  Valid before
+        or after the first inference."""
+        self._engine.set_memory_efficient_attention(True)
+
+    def disable_xformers_memory_efficient_attention(self):
+        """Back to the default: the high-precision mode stores the score matrices (the plans ``bench.py`` measures)."""
+        self._engine.set_memory_efficient_attention(False)
 
     def set_progress_bar_config(self, **k):
         return None

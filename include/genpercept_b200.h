@@ -77,6 +77,13 @@ gp_status gp_plan(gp_engine* e, int batch, int height, int width);
 
 /* number of cached plans (the cache is bounded: least-recently-used plans are destroyed; GP_MAX_PLANS, default 4) */
 int gp_plan_count(gp_engine* e);
+/* replaces: pipe.enable_xformers_memory_efficient_attention() / disable_... (run.py:382-385, infer.py:400-403).
+ * enable != 0: in the high-precision mode (gp_config.precision = 1) every self-attention (head_dim 64) and VAE mid-block
+ * attention (head_dim 512) runs fused, so no T x T score matrix is stored and a plan's memory grows with the pixel count.
+ * Off by default: the high-precision plans then store the score matrices, and a shape whose rows exceed the unfused
+ * softmax's 16384 keys fails at gp_plan with GP_ERR_INVALID.  The 16-bit modes always bound the score matrix and ignore
+ * the switch.  Valid before or after gp_finalize; a change of value drops the cached plans. */
+gp_status gp_set_memory_efficient_attention(gp_engine* e, int enable);
 /* Host-only introspection (no device needed): the N tile (BN) and the number of 128-pixel M tiles per CTA (MT) the planner
  * gives a stride-1 ks x ks convolution / linear layer cin -> cout over `images` maps of h x w output pixels on a GPU with
  * num_sms SMs (tokens_mode != 0: one row of images * h * w tokens).  Nothing in the reference corresponds to it (PyTorch /
@@ -156,6 +163,13 @@ gp_status gp_layernorm(int dtype, const void* x, int64_t tokens, int C, const fl
 /* softmax(q k^T * scale) v per (batch, head); q,k,v,o: 16-bit [B,T,heads*d] */
 gp_status gp_attention(int dtype, const void* q, const void* k, const void* v, int B, int T, int heads, int d,
                        float scale, void* o, void* stream);
+/* replaces: the fp32 attention of the reference's default dtype, in the engine's high-precision layout (fp16 (hi, lo)
+ * pairs, value = hi + lo).  softmax(q k^T) v per (batch, head), the softmax scale already folded into q as the engine folds
+ * it into Wq.  qk: [B,T,4C] = per token [q hi | k hi | q lo | k lo] (C = heads * d each); v: [B,T,2C] = [v hi | v lo];
+ * o: [B,T,2C] = [o hi | o lo].  d = 64 or (heads = 1) 512.  fused != 0: the fused split-precision kernel; 0: the unfused
+ * QK^T -> softmax -> P V path (GP_ERR_INVALID where its softmax cannot take rows of T keys).  V^T goes through the
+ * engine's own GEMM either way. */
+gp_status gp_attention_high(const void* qk, const void* v, int B, int T, int heads, int d, int fused, void* o, void* stream);
 /* replaces: the align / reduce / normalise tail of ensemble_depth (/root/reference/genpercept/util/ensemble.py:101-156,
  * 186-203): out[H,W] = median (torch.median: lower middle) or mean over the B <= 32 members of pred[b] * scale[b] + shift[b],
  * then (normalise 1) (x - min) / max(max - min, 1e-6) or (normalise 2) x / max(max, 1e-6).  pred / out: fp32 on the device. */
@@ -187,6 +201,10 @@ gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int k
  * kernel, 0 the unfused QK^T -> softmax -> P V path, whichever the planner would pick for that size.  Returns the
  * average microseconds over `iters` calls after one warm-up call, and the algorithmic FLOPs (4 B T^2 512) of one call. */
 gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, double* usec, double* flops);
+/* time one path of the high-precision attention (as gp_attention_high) on B images of T tokens, `heads` heads of d = 64
+ * or one of d = 512: fused != 0 the fused split-precision kernel, 0 the unfused path (GP_ERR_INVALID where it cannot run).
+ * Returns the average microseconds over `iters` calls after one warm-up call, and the algorithmic FLOPs (4 B heads T^2 d). */
+gp_status gp_bench_attention_high(int B, int T, int heads, int d, int fused, int iters, double* usec, double* flops);
 
 #ifdef __cplusplus
 }
