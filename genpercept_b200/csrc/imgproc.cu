@@ -18,7 +18,7 @@
 #include <tuple>
 #include <vector>
 
-#include "../../include/genpercept_b200.h"
+#include "prepost.h"
 
 namespace gp {
 namespace {
@@ -75,14 +75,11 @@ void build_axis(int in_size, int out_size, int mode, std::vector<int>& xmin, std
   *kmax_out = kmax;
 }
 
-std::mutex g_mu;
 std::map<std::tuple<int, int, int, int>, AxisTable> g_tables;     // (device, in, out, mode)
 struct Scratch { void* p = nullptr; size_t bytes = 0; };
 std::map<int, Scratch> g_scratch;                                   // per device, grows
 
-void ck(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
-}
+void ck(cudaError_t e, const char* what) { prepost_ck(e, what); }
 
 const AxisTable& axis_table(int dev, int in_size, int out_size, int mode) {
   auto key = std::make_tuple(dev, in_size, out_size, mode);
@@ -106,18 +103,6 @@ const AxisTable& axis_table(int dev, int in_size, int out_size, int mode) {
   ck(cudaMemcpy(t.xsize, xsize.data(), xsize.size() * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
   ck(cudaMemcpy(t.w, w.data(), w.size() * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
   return g_tables.emplace(key, t).first->second;
-}
-
-void* scratch(int dev, size_t bytes) {
-  Scratch& s = g_scratch[dev];
-  if (s.bytes < bytes) {
-    if (s.p) ck(cudaFree(s.p), "cudaFree");
-    s.p = nullptr;
-    s.bytes = 0;
-    ck(cudaMalloc(&s.p, bytes), "cudaMalloc");
-    s.bytes = bytes;
-  }
-  return s.p;
 }
 
 __device__ __forceinline__ float ldf(const uint8_t* p, long long i) { return (float)p[i]; }
@@ -203,23 +188,27 @@ int grid_for(long long n, int dev) {
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
-template <typename F>
-gp_status guarded(F f) {
-  try {
-    f();
-    return GP_OK;
-  } catch (const std::invalid_argument& ex) {
-    fprintf(stderr, "[genpercept_b200] %s\n", ex.what());
-    return GP_ERR_INVALID;
-  } catch (const std::exception& ex) {
-    fprintf(stderr, "[genpercept_b200] %s\n", ex.what());
-    return GP_ERR_CUDA;
-  }
-}
-
 size_t esize(int dtype) { return dtype == GP_U8 ? 1 : 4; }
 
 }  // namespace
+
+std::mutex& prepost_mutex() {
+  static std::mutex mu;
+  return mu;
+}
+
+void* prepost_scratch(int dev, size_t bytes) {
+  Scratch& s = g_scratch[dev];
+  if (s.bytes < bytes) {
+    if (s.p) ck(cudaFree(s.p), "cudaFree");
+    s.p = nullptr;
+    s.bytes = 0;
+    ck(cudaMalloc(&s.p, bytes), "cudaMalloc");
+    s.bytes = bytes;
+  }
+  return s.p;
+}
+
 }  // namespace gp
 
 using namespace gp;
@@ -228,11 +217,11 @@ extern "C" {
 
 gp_status gp_resize_aa(const void* src, int src_dtype, int src_on_host, int N, int H, int W, void* dst, int dst_dtype,
                        int dst_on_host, int OH, int OW, int mode, void* stream) {
-  return guarded([&]() {
+  return prepost_guarded([&]() {
     if (!src || !dst || N < 1 || H < 1 || W < 1 || OH < 1 || OW < 1 || (mode != 0 && mode != 1) ||
         (src_dtype != GP_U8 && src_dtype != GP_F32) || (dst_dtype != GP_U8 && dst_dtype != GP_F32))
       throw std::invalid_argument("gp_resize_aa: bad arguments");
-    std::lock_guard<std::mutex> lock(g_mu);
+    std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
     ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -241,7 +230,7 @@ gp_status gp_resize_aa(const void* src, int src_dtype, int src_on_host, int N, i
     const size_t in_b = src_on_host ? (n_in * esize(src_dtype) + 255) / 256 * 256 : 0;
     const size_t mid_b = (n_mid * 4 + 255) / 256 * 256;
     const size_t out_b = dst_on_host ? (n_out * esize(dst_dtype) + 255) / 256 * 256 : 0;
-    uint8_t* sc = static_cast<uint8_t*>(scratch(dev, in_b + mid_b + out_b));
+    uint8_t* sc = static_cast<uint8_t*>(prepost_scratch(dev, in_b + mid_b + out_b));
     const void* d_src = src;
     if (src_on_host) {
       ck(cudaMemcpyAsync(sc, src, n_in * esize(src_dtype), cudaMemcpyHostToDevice, s), "H2D");
@@ -279,17 +268,17 @@ gp_status gp_resize_aa(const void* src, int src_dtype, int src_on_host, int N, i
 
 gp_status gp_colorize(const float* pred, int pred_on_host, int B, int H, int W, float vmin, float vmax,
                       const uint8_t* lut768_host, uint8_t* out_hwc, int out_on_host, void* stream) {
-  return guarded([&]() {
+  return prepost_guarded([&]() {
     if (!pred || !lut768_host || !out_hwc || B < 1 || H < 1 || W < 1 || !(vmax > vmin))
       throw std::invalid_argument("gp_colorize: bad arguments");
-    std::lock_guard<std::mutex> lock(g_mu);
+    std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
     ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const size_t n = (size_t)B * H * W;
     const size_t in_b = pred_on_host ? (n * 4 + 255) / 256 * 256 : 0;
     const size_t out_b = out_on_host ? (n * 3 + 255) / 256 * 256 : 0;
-    uint8_t* sc = static_cast<uint8_t*>(scratch(dev, 1024 + in_b + out_b));
+    uint8_t* sc = static_cast<uint8_t*>(prepost_scratch(dev, 1024 + in_b + out_b));
     ck(cudaMemcpyAsync(sc, lut768_host, 768, cudaMemcpyHostToDevice, s), "lut H2D");
     const float* d_pred = pred;
     if (pred_on_host) {
@@ -305,16 +294,16 @@ gp_status gp_colorize(const float* pred, int pred_on_host, int B, int H, int W, 
 }
 
 gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, void* out, int out_on_host, void* stream) {
-  return guarded([&]() {
+  return prepost_guarded([&]() {
     if (!pred || !out || n < 1 || (bits != 8 && bits != 16)) throw std::invalid_argument("gp_quantize: bad arguments");
-    std::lock_guard<std::mutex> lock(g_mu);
+    std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
     ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const size_t ob = bits / 8;
     const size_t in_b = pred_on_host ? (n * 4 + 255) / 256 * 256 : 0;
     const size_t out_b = out_on_host ? (n * ob + 255) / 256 * 256 : 0;
-    uint8_t* sc = (in_b + out_b) ? static_cast<uint8_t*>(scratch(dev, in_b + out_b)) : nullptr;
+    uint8_t* sc = (in_b + out_b) ? static_cast<uint8_t*>(prepost_scratch(dev, in_b + out_b)) : nullptr;
     const float* d_pred = pred;
     if (pred_on_host) {
       ck(cudaMemcpyAsync(sc, pred, n * 4, cudaMemcpyHostToDevice, s), "H2D");

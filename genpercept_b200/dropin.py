@@ -12,12 +12,20 @@ that exports this package's classes makes the unmodified ``run.py`` / ``infer.py
 
 or, from Python, ``import genpercept_b200.dropin; genpercept_b200.dropin.install()`` before the first
 ``import genpercept``.
+
+For ``eval.py`` (and only for it) the drop-in also seeds ``sys.modules["src.util.alignment"]`` and
+``sys.modules["src.util.metric"]`` with ``genpercept_b200.evaluation``, so eval.py's ``from src.util import metric``,
+``getattr(metric, name)``, ``MetricTracker`` and ``align_depth_least_square`` run on the GPU while ``src.dataset`` keeps
+coming from the reference checkout:
+
+    PYTHONPATH=/path/to/genpercept_b200_repo python -m genpercept_b200.dropin eval.py --prediction_dir ... --alignment ...
 """
 import runpy
 import sys
 import types
 
 _NAME = "genpercept.genpercept_pipeline"
+_EVAL_NAMES = ("src.util.alignment", "src.util.metric")
 
 
 def install():
@@ -39,14 +47,27 @@ def install():
     return mod
 
 
+def install_evaluation():
+    """Idempotent.  Seeds src.util.alignment / src.util.metric with genpercept_b200.evaluation; returns it."""
+    from . import evaluation
+    for name in _EVAL_NAMES:
+        sys.modules[name] = evaluation
+        parent = sys.modules.get("src.util")
+        if parent is not None:        # src.util was imported first: rebind its submodule attributes too
+            setattr(parent, name.rsplit(".", 1)[1], evaluation)
+    return evaluation
+
+
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     if not argv:
-        sys.exit("usage: python -m genpercept_b200.dropin <run.py|infer.py> [its arguments ...]")
+        sys.exit("usage: python -m genpercept_b200.dropin <run.py|infer.py|eval.py> [its arguments ...]")
     install()
     script = argv[0]
-    sys.argv = argv
     import os
+    if os.path.basename(script) == "eval.py":
+        install_evaluation()
+    sys.argv = argv
     sys.path.insert(0, os.path.dirname(os.path.abspath(script)))      # what `python script.py` would have done
     runpy.run_path(script, run_name="__main__")
 

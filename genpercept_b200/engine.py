@@ -87,6 +87,10 @@ def lib():
     L.gp_colorize.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_int,
                               c_void_p]
     L.gp_quantize.argtypes = [c_void_p, c_int, c_size_t, c_int, c_void_p, c_int, c_void_p]
+    L.gp_depth_align.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                 c_void_p]
+    L.gp_depth_metrics.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_float,
+                                   c_void_p, c_void_p]
     _lib = L
     return L
 
@@ -466,6 +470,33 @@ def quantize(pred, bits=16, to_host=True):
     st = lib().gp_quantize(c_void_p(pred.data_ptr()), 0 if pred.is_cuda else 1, pred.numel(), bits, ptr, on_host,
                            _stream_ptr())
     _check_free(st, "gp_quantize")
+    return out
+
+
+def _ptr(t):
+    return None if t is None else c_void_p(t.data_ptr())
+
+
+def depth_align(pred, gt, valid, mode=0, max_res=0, aligned=False):
+    """gp_depth_align: pred / gt contiguous cuda fp32 [B,H,W], valid cuda uint8 [B,H,W] or None (all valid); mode 0
+    (fit gt) or 1 (disparity of gt).  Returns (scale_shift fp32 [B,2], aligned fp32 [B,H,W] or None), on the device."""
+    B, H, W = pred.shape
+    ss = torch.empty((B, 2), dtype=torch.float32, device=pred.device)
+    out = torch.empty_like(pred) if aligned else None
+    st = lib().gp_depth_align(_ptr(pred), _ptr(gt), _ptr(valid), B, H, W, int(mode), int(max_res), _ptr(ss), _ptr(out),
+                              _stream_ptr(pred.device))
+    _check_free(st, "gp_depth_align")
+    return ss, out
+
+
+def depth_metrics(pred, gt, valid, mode=0, scale_shift=None, min_depth=0.0, max_depth=1e8):
+    """gp_depth_metrics: the ten eval.py metrics per image -> fp64 [B,10] on the device.  mode 0 none, 1 least squares,
+    2 least squares in disparity (scale_shift fp32 [B,2] on the device)."""
+    B, H, W = pred.shape
+    out = torch.empty((B, 10), dtype=torch.float64, device=pred.device)
+    st = lib().gp_depth_metrics(_ptr(pred), _ptr(gt), _ptr(valid), B, H, W, int(mode), _ptr(scale_shift), float(min_depth),
+                                float(max_depth), _ptr(out), _stream_ptr(pred.device))
+    _check_free(st, "gp_depth_metrics")
     return out
 
 

@@ -193,6 +193,24 @@ gp_status gp_colorize(const float* pred, int pred_on_host, int B, int H, int W, 
                       const uint8_t* lut768_host, uint8_t* out_hwc, int out_on_host, void* stream);
 /* (pred*255).astype(uint8) / (pred*65535).astype(uint16) of /root/reference/run.py:449-455; bits = 8 or 16. */
 gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, void* out, int out_on_host, void* stream);
+/* ---- depth evaluation (SURVEY.md §8 f4): the reference's eval.py loop on the device; engine-free ------------------
+ * pred, gt: fp32 [B,H,W]; valid: uint8 [B,H,W] (nonzero = valid; NULL = every pixel); all device pointers.  Both
+ * calls use the pre/post scratch buffer above, return asynchronously on `stream`, and are bit-identical run to run.
+ * gp_depth_align replaces align_depth_least_square (/root/reference/src/util/alignment.py:29-76): per image the
+ * (scale, shift) np.linalg.lstsq fits to gt over the valid pixels, rounded to float32 -> scale_shift_out [B,2] (device).
+ * mode 0 fits gt as given; 1 the disparity mode of eval.py:177-197 (target 1/gt where gt > 0, mask valid & gt > 0 &
+ * pred > 0).  max_res > 0: the fit reads the grid torch.nn.Upsample(scale_factor=min(max_res/(H,W)), "nearest") makes
+ * of the [1,H,W] map when that factor is below 1 (a 1-D resample: H x floor(W*s)); 0 = none.  No pixel valid -> (0, 0);
+ * a constant prediction -> lstsq's minimum-norm solution.  aligned_out (nullable): fp32 [B,H,W] pred*scale + shift. */
+gp_status gp_depth_align(const float* pred, const float* gt, const uint8_t* valid, int B, int H, int W, int mode,
+                         int max_res, float* scale_shift_out, float* aligned_out, void* stream);
+/* The ten metrics of eval.py:42-53 per image -> metrics_out fp64 [B,10] (device), in that order: abs_relative_difference,
+ * squared_relative_difference, rmse_linear, rmse_log, log10, delta1_acc, delta2_acc, delta3_acc, i_rmse, silog_rmse.
+ * Per pixel (float32, eval.py:168-205): mode 0 pred as given; 1 pred*scale+shift; 2 the same, clipped at 1e-3 and
+ * inverted (disparity -> depth); then clip to [min_depth, max_depth] and to >= 1e-6.  scale_shift: [B,2] on the device
+ * (gp_depth_align's output; unused in mode 0).  No pixel valid -> NaN metrics, like the reference. */
+gp_status gp_depth_metrics(const float* pred, const float* gt, const uint8_t* valid, int B, int H, int W, int mode,
+                           const float* scale_shift, float min_depth, float max_depth, double* metrics_out, void* stream);
 
 /* time one igemm configuration: returns average microseconds over `iters` launches */
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters,
