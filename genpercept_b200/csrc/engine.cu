@@ -41,6 +41,9 @@ struct Plan {
   std::map<int, cudaGraphExec_t> graphs;   // by out_channels
   double igemm_flops = 0;
   int eager_runs = 0;                       // the first pass runs eagerly (kernel attributes, lazy init), then graphs
+  // gp_infer_latent's UNet -> readout range: its own graphs and first eager pass, so the full pipeline's stay as they are
+  std::map<int, cudaGraphExec_t> latent_graphs;
+  int latent_eager_runs = 0;
   int64_t launches = 0;
 };
 
@@ -62,6 +65,7 @@ struct gp_engine {
   void drop_plan(std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>>::iterator it) {
     GP_CUDA(cudaDeviceSynchronize());
     for (auto& g : it->second->graphs) cudaGraphExecDestroy(g.second);
+    for (auto& g : it->second->latent_graphs) cudaGraphExecDestroy(g.second);
     if (it->second->arena) cudaFree(it->second->arena);
     if (cur == it->second.get()) cur = nullptr;
     plans.erase(it);
@@ -595,6 +599,45 @@ void stage_rgb(gp_engine* e, Plan* p, const void* rgb, int rgb_dtype, int rgb_on
   GP_CUDA(preprocess_rgb_im2col(src, kind, p->arena + p->kept["rgb"].t.off, p->B, p->H, p->W, e->ws.bf16, s, e->ws.split));
 }
 
+// Runs the ops of stages `first` .. GP_STAGE_READOUT and delivers the result to `out` (device, or host if out_on_host).
+// The first pass through an entry point runs eagerly (`eager_runs`); with CUDA graphs on, later passes replay the graph
+// captured in `graphs` for out_channels.
+void run_to_out(gp_engine* e, Plan* p, int first, std::map<int, cudaGraphExec_t>& graphs, int& eager_runs, float* out,
+                int out_on_host, int out_channels, cudaStream_t s) {
+  const size_t npix_out = (size_t)p->B * p->outH * p->outW;
+  // 2 = auto: replay a graph where the launch stream is the bottleneck — small plans
+  const bool use_graph = e->cfg.use_cuda_graph == 1 ||
+                         (e->cfg.use_cuda_graph == 2 && (long long)p->B * p->H * p->W <= 2LL * 768 * 768);
+  // eager launches write the result straight into a device `out`; a captured graph has the plan's own buffer baked in
+  const bool graph_now = use_graph && eager_runs > 0;
+  p->out_dst = (graph_now || out_on_host) ? p->out_f32 : out;
+  if (graph_now) {
+    auto it = graphs.find(out_channels);
+    if (it == graphs.end()) {
+      cudaStream_t cs;
+      GP_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+      cudaGraph_t g;
+      GP_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+      cudaError_t re = run_ops(p, first, GP_STAGE_READOUT, out_channels, cs);
+      cudaError_t ce = cudaStreamEndCapture(cs, &g);
+      cudaStreamDestroy(cs);
+      GP_CUDA(re);
+      GP_CUDA(ce);
+      cudaGraphExec_t ge;
+      GP_CUDA(cudaGraphInstantiate(&ge, g, 0));
+      cudaGraphDestroy(g);
+      it = graphs.emplace(out_channels, ge).first;
+    }
+    GP_CUDA(cudaGraphLaunch(it->second, s));
+  } else {
+    GP_CUDA(run_ops(p, first, GP_STAGE_READOUT, out_channels, s));
+    eager_runs++;
+  }
+  if (p->out_dst != out)
+    GP_CUDA(cudaMemcpyAsync(out, p->out_f32, npix_out * out_channels * 4, out_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, s));
+  p->out_dst = p->out_f32;
+}
+
 }  // namespace
 
 extern "C" {
@@ -624,6 +667,7 @@ void gp_destroy(gp_engine* e) {
   if (!e) return;
   for (auto& kv : e->plans) {
     for (auto& g : kv.second->graphs) cudaGraphExecDestroy(g.second);
+    for (auto& g : kv.second->latent_graphs) cudaGraphExecDestroy(g.second);
     if (kv.second->arena) cudaFree(kv.second->arena);
   }
   delete e;
@@ -767,40 +811,34 @@ gp_status gp_infer(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
     p->last_used = ++e->use_clock;
-    const size_t npix_out = (size_t)p->B * p->outH * p->outW;
     stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_infer");
-    // 2 = auto: replay a graph where the launch stream is the bottleneck — small plans
-    const bool use_graph = e->cfg.use_cuda_graph == 1 ||
-                           (e->cfg.use_cuda_graph == 2 && (long long)p->B * p->H * p->W <= 2LL * 768 * 768);
-    // eager launches write the result straight into a device `out`; a captured graph has the plan's own buffer baked in
-    const bool graph_now = use_graph && p->eager_runs > 0;
-    p->out_dst = (graph_now || out_on_host) ? p->out_f32 : out;
-    if (graph_now) {
-      auto it = p->graphs.find(out_channels);
-      if (it == p->graphs.end()) {
-        cudaStream_t cs;
-        GP_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        cudaGraph_t g;
-        GP_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-        cudaError_t re = run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_READOUT, out_channels, cs);
-        cudaError_t ce = cudaStreamEndCapture(cs, &g);
-        cudaStreamDestroy(cs);
-        GP_CUDA(re);
-        GP_CUDA(ce);
-        cudaGraphExec_t ge;
-        GP_CUDA(cudaGraphInstantiate(&ge, g, 0));
-        cudaGraphDestroy(g);
-        it = p->graphs.emplace(out_channels, ge).first;
-      }
-      GP_CUDA(cudaGraphLaunch(it->second, s));
-    } else {
-      GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_READOUT, out_channels, s));
-      p->eager_runs++;
-    }
-    if (p->out_dst != out)
-      GP_CUDA(cudaMemcpyAsync(out, p->out_f32, npix_out * out_channels * 4, out_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, s));
-    p->out_dst = p->out_f32;
+    run_to_out(e, p, GP_STAGE_VAE_ENCODE, p->graphs, p->eager_runs, out, out_on_host, out_channels, s);
     if (rgb_on_host || out_on_host) GP_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+gp_status gp_infer_latent(gp_engine* e, const float* latent_dev, int batch, int channels, int height, int width, float* out,
+                          int out_on_host, int out_channels, void* stream) {
+  return guarded(e, [&]() {
+    if (e->multistep) throw GpError(GP_ERR_INVALID, "gp_infer_latent: runs the one-step arch only (gp_config.arch = 0)");
+    Plan* p = e->cur;
+    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_infer_latent: no plan (call gp_plan)");
+    if (e->cfg.readout == GP_READOUT_DPT) out_channels = 1;
+    GP_REQUIRE(latent_dev && out && (out_channels == 1 || out_channels == 3), "gp_infer_latent: bad arguments");
+    const T4& lat = p->kept["rgb_latent"].t;
+    const int lat_c = e->ws.split ? 8 : 4;
+    GP_REQUIRE(batch == lat.N && channels == lat_c && height == lat.H && width == lat.W,
+               "gp_infer_latent: latent [" + std::to_string(batch) + "," + std::to_string(channels) + "," + std::to_string(height) +
+                   "," + std::to_string(width) + "] does not match the plan's [" + std::to_string(lat.N) + "," +
+                   std::to_string(lat_c) + "," + std::to_string(lat.H) + "," + std::to_string(lat.W) + "]" +
+                   (e->ws.split ? " (the high-precision mode takes the (hi, lo) pair gp_encode_exact writes)" : ""));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    p->last_used = ++e->use_clock;
+    if (e->ws.split) GP_CUDA(latent_pair_from_nchw(latent_dev, p->arena + lat.off, lat.N, lat.H, lat.W, e->ws.bf16, s));
+    else GP_CUDA(nchw4_affine_to_nhwc8(latent_dev, p->arena + lat.off, lat.N, lat.H, lat.W, 1.0f, nullptr, nullptr, e->ws.bf16, s));
+    run_to_out(e, p, GP_STAGE_UNET, p->latent_graphs, p->latent_eager_runs, out, out_on_host, out_channels, s);
+    if (out_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }
 
@@ -815,6 +853,22 @@ gp_status gp_encode(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_hos
     GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, 1, s));
     const T4& l = p->kept["rgb_latent"].t;
     GP_CUDA(nhwc8_to_nchw_f32(p->arena + l.off, latent_dev, l.N, l.H, l.W, 4, e->ws.bf16, s, e->ws.split));
+    if (rgb_on_host) GP_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+gp_status gp_encode_exact(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, float* latent_dev, void* stream) {
+  if (e && !e->ws.split) return gp_encode(e, rgb, rgb_dtype, rgb_on_host, latent_dev, stream);
+  return guarded(e, [&]() {
+    Plan* p = e->cur;
+    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_encode_exact: no plan (call gp_plan)");
+    GP_REQUIRE(rgb && latent_dev, "gp_encode_exact: bad arguments");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_encode_exact");
+    GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, 1, s));
+    const T4& l = p->kept["rgb_latent"].t;
+    GP_CUDA(latent_pair_to_nchw(p->arena + l.off, latent_dev, l.N, l.H, l.W, e->ws.bf16, s));
     if (rgb_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }

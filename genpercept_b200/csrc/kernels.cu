@@ -985,8 +985,10 @@ cudaError_t softmax_rows(void* sio, long long rows, int T, int Tp, bool bf16, cu
       cudaGetDevice(&dev);
       if (!sms[dev & 63]) {
         cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
-        GP_DISPATCH_BF16(bf16, (cudaFuncSetAttribute(softmax_rows_pipe_kernel<BF, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)));
-        GP_DISPATCH_BF16(bf16, (cudaFuncSetAttribute(softmax_rows_pipe_kernel<BF, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)));
+        // the flag is per device, so both storage types get the attribute: an fp16 engine may come first in a process
+        for (const void* f : {(const void*)softmax_rows_pipe_kernel<false, 3>, (const void*)softmax_rows_pipe_kernel<false, 6>,
+                              (const void*)softmax_rows_pipe_kernel<true, 3>, (const void*)softmax_rows_pipe_kernel<true, 6>})
+          cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
       }
       int per_sm = (220 * 1024) / (smem + 1024);
       if (per_sm > 5) per_sm = 5;                 // 5 x 384 threads
@@ -1037,9 +1039,11 @@ cudaError_t xattn2(const void* x, void* y, long long tokens, int C, int heads, c
     cudaGetDevice(&dev);
     if (!sms[dev & 63]) {
       const int big = 226 * 1024;
-      GP_DISPATCH_BF16(bf16, (cudaFuncSetAttribute(xattn2_smem_kernel<BF, 2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, big)));
-      GP_DISPATCH_BF16(bf16, (cudaFuncSetAttribute(xattn2_smem_kernel<BF, 3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, big)));
-      GP_DISPATCH_BF16(bf16, (cudaFuncSetAttribute(xattn2_smem_kernel<BF, 5, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, big)));
+      // the flag is per device, so both storage types get the attribute: an fp16 engine may come first in a process
+      for (const void* f : {(const void*)xattn2_smem_kernel<false, 2, 2>, (const void*)xattn2_smem_kernel<false, 3, 2>,
+                            (const void*)xattn2_smem_kernel<false, 5, 1>, (const void*)xattn2_smem_kernel<true, 2, 2>,
+                            (const void*)xattn2_smem_kernel<true, 3, 2>, (const void*)xattn2_smem_kernel<true, 5, 1>})
+        cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, big);
       cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
     }
     int per_sm = (int)((227 * 1024) / (smem + 1024));
@@ -1125,6 +1129,38 @@ __global__ void nchw4_affine_to_nhwc8_kernel(const float* __restrict__ in, uint1
     }
   }
   store8<BF16>(out + i * (lo ? 16 : 8), lo, f);
+}
+// A high-precision latent as its (hi, lo) pair: split NHWC8 (per pixel [hi 0..7 | lo 0..7]) <-> fp32 NCHW [N, 8, H, W] =
+// [hi 0..3 | lo 0..3].  Every 16-bit value is exact in fp32, so the pair survives the round trip bit for bit; the fp32
+// sum hi + lo does not determine it (where lo rounded to half an ulp of hi, re-splitting ties to even and can pick the
+// other neighbour).  The import writes zeros to channels 4..7 of both planes, as the encoder's tail does.
+template <bool BF16>
+__global__ void latent_pair_to_nchw_kernel(const uint16_t* __restrict__ in, float* __restrict__ out, int N, long long HW) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)N * HW) return;
+  float* o = out + (long long)(i / HW) * 8 * HW + i % HW;
+  float h[8], l[8];
+  unpack8<BF16>(*reinterpret_cast<const uint4*>(in + i * 16), h);
+  unpack8<BF16>(*reinterpret_cast<const uint4*>(in + i * 16 + 8), l);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    o[k * HW] = h[k];
+    o[(4 + k) * HW] = l[k];
+  }
+}
+template <bool BF16>
+__global__ void latent_pair_from_nchw_kernel(const float* __restrict__ in, uint16_t* __restrict__ out, int N, long long HW) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)N * HW) return;
+  const float* x = in + (long long)(i / HW) * 8 * HW + i % HW;
+  float h[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, l[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    h[k] = x[k * HW];
+    l[k] = x[(4 + k) * HW];
+  }
+  *reinterpret_cast<uint4*>(out + i * 16) = pack8<BF16>(h);
+  *reinterpret_cast<uint4*>(out + i * 16 + 8) = pack8<BF16>(l);
 }
 }  // namespace
 
@@ -1220,6 +1256,20 @@ cudaError_t nchw4_affine_to_nhwc8(const float* in, void* out, int N, int H, int 
   const long long HW = (long long)H * W, total = (long long)N * HW;
   GP_DISPATCH_BF16(bf16, (launch(nchw4_affine_to_nhwc8_kernel<BF>, (unsigned)((total + 255) / 256), 256, 0, s, 
                              in, reinterpret_cast<uint16_t*>(out), N, HW, pre, m, b, split ? 8 : 0)));
+  return cudaGetLastError();
+}
+
+cudaError_t latent_pair_to_nchw(const void* in, float* out, int N, int H, int W, bool bf16, cudaStream_t s) {
+  const long long HW = (long long)H * W, total = (long long)N * HW;
+  GP_DISPATCH_BF16(bf16, (launch(latent_pair_to_nchw_kernel<BF>, (unsigned)((total + 255) / 256), 256, 0, s,
+                             reinterpret_cast<const uint16_t*>(in), out, N, HW)));
+  return cudaGetLastError();
+}
+
+cudaError_t latent_pair_from_nchw(const float* in, void* out, int N, int H, int W, bool bf16, cudaStream_t s) {
+  const long long HW = (long long)H * W, total = (long long)N * HW;
+  GP_DISPATCH_BF16(bf16, (launch(latent_pair_from_nchw_kernel<BF>, (unsigned)((total + 255) / 256), 256, 0, s,
+                             in, reinterpret_cast<uint16_t*>(out), N, HW)));
   return cudaGetLastError();
 }
 

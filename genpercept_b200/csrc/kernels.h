@@ -72,6 +72,9 @@ cudaError_t bilinear_resize(const void* in, void* out, int N, int H, int W, int 
 cudaError_t nhwc8_to_nchw_f32(const void* in, float* out, int N, int H, int W, int c, bool bf16, cudaStream_t s, bool split = false);
 cudaError_t nchw4_affine_to_nhwc8(const float* in, void* out, int N, int H, int W, float pre, const float* m /*[4][4] or null*/,
                                   const float* b /*[4] or null*/, bool bf16, cudaStream_t s, bool split = false);
+// the high-precision latent's (hi, lo) pair without loss: split NHWC8 <-> fp32 NCHW [N,8,H,W] = [hi 0..3 | lo 0..3]
+cudaError_t latent_pair_to_nchw(const void* in, float* out, int N, int H, int W, bool bf16, cudaStream_t s);
+cudaError_t latent_pair_from_nchw(const float* in, void* out, int N, int H, int W, bool bf16, cudaStream_t s);
 // u8 / f16 / f32 NCHW [N,3,H,W] (u8 is mapped x/255*2-1), K-packed for the VAE encoder's stem: 16-bit NHWC32 = the pixel's
 // 3x3 neighbourhood along the channel axis [centre tap | 8 other taps row-major | 5 zeros]; im2col_tap_slot(r, q) gives a
 // tap's position.

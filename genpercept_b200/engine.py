@@ -51,6 +51,8 @@ def lib():
     L.gp_run_stage.argtypes = [c_void_p, c_int, c_int, c_void_p]
     L.gp_encode.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
     L.gp_decode.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]
+    L.gp_encode_exact.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
+    L.gp_infer_latent.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]
     L.gp_set_timestep.argtypes = [c_void_p, c_int]
     L.gp_infer_steps.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, POINTER(c_int), POINTER(c_float), c_int, c_void_p,
                                  c_int, c_int, c_void_p]
@@ -232,6 +234,38 @@ class Engine:
             f"out must be contiguous fp32 {(B, C, Ho, Wo)}"
         self._ck(self.L.gp_infer(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), 0 if rgb.is_cuda else 1,
                                  c_void_p(out.data_ptr()), 0 if out.is_cuda else 1, C, self._sp()), "gp_infer")
+        return out
+
+    def encode_exact(self, rgb):
+        """The latent ``infer_latent`` takes, without loss (gp_encode_exact): [B,3,H,W] uint8 / float -> fp32
+        [B,4,H/8,W/8] (cuda) in the 16-bit modes, the same as ``encode``; in the high-precision mode fp32 [B,8,H/8,W/8] =
+        [hi | lo], the (hi, lo) pair of every value.  Plans (B, H, W) like ``infer``."""
+        B, _, H, W = rgb.shape
+        if self.plan_shape != (B, H, W):
+            self.plan(B, H, W)
+        rgb = (rgb.float() if rgb.dtype == torch.bfloat16 else rgb).contiguous()
+        c = 8 if self.precision == "high" else 4
+        lat = torch.empty((B, c) + self.tensor_shape("rgb_latent")[2:], dtype=torch.float32, device=self.device)
+        self._ck(self.L.gp_encode_exact(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), 0 if rgb.is_cuda else 1,
+                                        c_void_p(lat.data_ptr()), self._sp()), "gp_encode_exact")
+        return lat
+
+    def infer_latent(self, latent, out_channels=1, out=None):
+        """``infer`` from the UNet on (gp_infer_latent): `latent` as ``encode_exact`` returns it, from this engine or another
+        with the same dtype, precision and VAE encoder.  It runs on the CURRENT plan, the one ``plan(B, H, W)`` (or
+        ``encode_exact`` / ``infer``) made for the image the latent came from: a latent's extent does not fix the image's,
+        and the image's sets the result's.  Returns fp32 [B,C,H,W] in [0,1] on the device of `out`, equal to ``infer``'s."""
+        assert latent.dim() == 4, "latent must be [B,C,h,w]"
+        B, c, h, w = latent.shape
+        latent = latent.to(self.device, torch.float32).contiguous()
+        C = 1 if self.readout == "dpt" else out_channels
+        Ho, Wo = self.out_hw if self.out_hw is not None else (0, 0)     # no plan: the library reports GP_ERR_NO_PLAN
+        if out is None:
+            out = torch.empty((B, C, Ho, Wo), dtype=torch.float32, device=self.device)
+        assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (B, C, Ho, Wo), \
+            f"out must be contiguous fp32 {(B, C, Ho, Wo)}"
+        self._ck(self.L.gp_infer_latent(self.h, c_void_p(latent.data_ptr()), B, c, h, w, c_void_p(out.data_ptr()),
+                                        0 if out.is_cuda else 1, C, self._sp()), "gp_infer_latent")
         return out
 
     def infer_steps(self, rgb, timesteps, coeffs, noise=None, out_channels=1, out=None):

@@ -129,6 +129,7 @@ class GenPerceptPipeline:
         self.device = self._engine.device
         unet_sd = dict(_as_state_dict(unet, variant))
         vae_sd = W.remap_legacy_vae_keys(_as_state_dict(vae, variant))
+        self._encoder_state = W.encoder_state(vae_sd)      # references, compared by multitask.MultiTaskPipeline
         if customized_head is not None:          # run.py:322-331 drops these for the DPT readout
             unet_sd = {k: v for k, v in unet_sd.items() if not k.startswith(("conv_out", "conv_norm_out"))}
             self._engine.load_state("dpt", _as_state_dict(customized_head))
@@ -219,11 +220,14 @@ class GenPerceptPipeline:
         if not self.genpercept_pipeline:
             return self._single_infer_steps(rgb_in, num_inference_steps, generator, fix_timesteps, prompt, mode)
         assert num_inference_steps == 1, "GenPercept only forward once."
+        return self._engine.infer(rgb_in, out_channels=self._one_step_setup(fix_timesteps, prompt, mode))
+
+    def _one_step_setup(self, fix_timesteps, prompt, mode):
+        """Readies the one-step engine for a call (text embedding, timestep); returns the map's channel count."""
         self._ensure_ready(prompt)
         # :405-408: a per-call fix_timesteps replaces the scheduler's [1] for THIS call only
         self._engine.set_timestep(int(fix_timesteps) if fix_timesteps else self._timestep)
-        ch = 1 if (self.customized_head is not None or self._mode(mode) in ONE_CHANNEL_MODES) else 3
-        return self._engine.infer(rgb_in, out_channels=ch)
+        return 1 if (self.customized_head is not None or self._mode(mode) in ONE_CHANNEL_MODES) else 3
 
     def _single_infer_steps(self, rgb_in, num_inference_steps, generator, fix_timesteps, prompt, mode):
         """genpercept_pipeline.py:399-472 with genpercept_pipeline=False: set_timesteps, pred_latent = randn (marigold) or
@@ -283,31 +287,7 @@ class GenPerceptPipeline:
             assert denoising_steps == 1
         else:
             assert denoising_steps >= 1
-        resample = get_tv_resample_method(resample_method)
-        if isinstance(input_image, Image.Image):
-            rgb = pil_to_tensor(input_image.convert("RGB")).unsqueeze(0)
-        elif isinstance(input_image, torch.Tensor):
-            rgb = input_image
-        else:
-            raise TypeError(f"Unknown input type: {type(input_image) = }")
-        input_size = rgb.shape
-        assert 4 == rgb.dim() and 3 == input_size[-3], f"Wrong input shape {input_size}, expected [1, rgb, H, W]"
-        # Pre/post-processing runs on the GPU (gp_resize_aa / gp_colorize / gp_quantize, SURVEY.md §8 f1) for the
-        # anti-aliased bilinear / bicubic filters; the nearest modes keep torchvision's host path.
-        gpu_resample = resample_method in E.RESIZE_MODES
-        if rgb.dtype != torch.uint8:
-            assert rgb.min() >= 0 and rgb.max() <= 255
-            rgb = rgb.float() if rgb.is_floating_point() else rgb.to(torch.uint8)
-        if processing_res > 0:
-            if gpu_resample:
-                h0, w0 = rgb.shape[-2:]
-                f = min(processing_res / w0, processing_res / h0)                    # image_util.py:98-102
-                rgb = E.resize_aa(rgb, int(h0 * f), int(w0 * f), resample_method, device=self.device)
-            else:
-                rgb = resize_max_res(rgb, max_edge_resolution=processing_res, resample_method=resample)
-        if rgb.dtype != torch.uint8:                       # float image in [0,255]: the reference keeps it float (:245)
-            rgb = rgb.to(self.device) / 255.0 * 2.0 - 1.0
-        # for uint8 the normalisation x/255*2-1 and the cast to self.dtype (:245-246) happen inside the engine
+        rgb, input_size = preprocess(input_image, processing_res, resample_method, self.device)
         if self.genpercept_pipeline or ensemble_size == 1:
             pred = self.single_infer(rgb, num_inference_steps=denoising_steps, generator=generator,
                                      show_pbar=show_progress_bar, fix_timesteps=fix_timesteps, prompt=prompt, mode=mode)
@@ -324,28 +304,65 @@ class GenPerceptPipeline:
                                                  prompt=prompt, mode=mode))
             pred, _ = ensemble_depth(torch.cat(members, dim=0), scale_invariant=True, shift_invariant=True, max_res=50,
                                      **(ensemble_kwargs or {}))
-        if match_input_res and tuple(pred.shape[-2:]) != tuple(input_size[-2:]):
-            if gpu_resample:
-                pred = E.resize_aa(pred, int(input_size[-2]), int(input_size[-1]), resample_method)
-            else:
-                pred = resize(pred, list(input_size[-2:]), interpolation=resample, antialias=True)
-        pred = pred.clamp(0, 1)                            # :310 (a bicubic resize can overshoot)
-        batched = pred.shape[0] > 1
-        one_ch = pred.shape[1] == 1
-        if color_map is not None:
-            assert self.mode in ["depth", "disparity"]
-            lut = (_lut(color_map) * 255).astype(np.uint8)                          # (c * 255).astype(uint8), :318-321
-            col = E.colorize(pred[:, 0].contiguous(), lut, 0.0, 1.0).numpy()      # [B,H,W,3] uint8 on the host
+        return postprocess(pred, input_size, match_input_res, resample_method, color_map, self.mode)
+
+
+# Pre/post-processing of ``__call__`` (shared with multitask.MultiTaskPipeline).  It runs on the GPU (gp_resize_aa /
+# gp_colorize / gp_quantize, SURVEY.md §8 f1) for the anti-aliased bilinear / bicubic filters; the nearest modes keep
+# torchvision's host path.
+def preprocess(input_image, processing_res, resample_method, device):
+    """The image intake of ``__call__``: a PIL image or a [B,3,H,W] tensor -> (the engine's rgb input, the input's
+    shape).  uint8 stays uint8 (the engine maps x/255*2-1 and casts, :245-246); a float image in [0,255] comes back
+    on `device` in [-1,1]."""
+    resample = get_tv_resample_method(resample_method)
+    if isinstance(input_image, Image.Image):
+        rgb = pil_to_tensor(input_image.convert("RGB")).unsqueeze(0)
+    elif isinstance(input_image, torch.Tensor):
+        rgb = input_image
+    else:
+        raise TypeError(f"Unknown input type: {type(input_image) = }")
+    input_size = rgb.shape
+    assert 4 == rgb.dim() and 3 == input_size[-3], f"Wrong input shape {input_size}, expected [1, rgb, H, W]"
+    if rgb.dtype != torch.uint8:
+        assert rgb.min() >= 0 and rgb.max() <= 255
+        rgb = rgb.float() if rgb.is_floating_point() else rgb.to(torch.uint8)
+    if processing_res > 0:
+        if resample_method in E.RESIZE_MODES:
+            h0, w0 = rgb.shape[-2:]
+            f = min(processing_res / w0, processing_res / h0)                    # image_util.py:98-102
+            rgb = E.resize_aa(rgb, int(h0 * f), int(w0 * f), resample_method, device=device)
         else:
-            col = E.quantize(pred, 8)                                               # (p * 255).astype(uint8)
-            col = col[:, 0] if one_ch else np.transpose(col, (0, 2, 3, 1))
-        colored = [Image.fromarray(c) for c in col]
-        pred_np = pred.cpu().numpy()
-        pred_np = pred_np.squeeze() if not batched else (pred_np[:, 0] if one_ch else pred_np)
-        if batched:
-            if pred_np.ndim == 4 and pred_np.shape[1] == 3:
-                pred_np = np.transpose(pred_np, (0, 2, 3, 1))
-            return GenPerceptOutput(pred_np=pred_np, pred_colored=colored)
-        if pred_np.ndim == 3 and pred_np.shape[0] == 3:
-            pred_np = np.transpose(pred_np, (1, 2, 0))
-        return GenPerceptOutput(pred_np=pred_np, pred_colored=colored[0])
+            rgb = resize_max_res(rgb, max_edge_resolution=processing_res, resample_method=resample)
+    if rgb.dtype != torch.uint8:                       # float image in [0,255]: the reference keeps it float (:245)
+        rgb = rgb.to(device) / 255.0 * 2.0 - 1.0
+    return rgb, input_size
+
+
+def postprocess(pred, input_size, match_input_res, resample_method, color_map, mode) -> GenPerceptOutput:
+    """The tail of ``__call__`` (:301-323): pred [B,C,h,w] in [0,1] -> resized back to `input_size`, clipped, and
+    colorized (`color_map`, depth / disparity) or quantized to uint8."""
+    if match_input_res and tuple(pred.shape[-2:]) != tuple(input_size[-2:]):
+        if resample_method in E.RESIZE_MODES:
+            pred = E.resize_aa(pred, int(input_size[-2]), int(input_size[-1]), resample_method)
+        else:
+            pred = resize(pred, list(input_size[-2:]), interpolation=get_tv_resample_method(resample_method), antialias=True)
+    pred = pred.clamp(0, 1)                            # :310 (a bicubic resize can overshoot)
+    batched = pred.shape[0] > 1
+    one_ch = pred.shape[1] == 1
+    if color_map is not None:
+        assert mode in ["depth", "disparity"]
+        lut = (_lut(color_map) * 255).astype(np.uint8)                          # (c * 255).astype(uint8), :318-321
+        col = E.colorize(pred[:, 0].contiguous(), lut, 0.0, 1.0).numpy()      # [B,H,W,3] uint8 on the host
+    else:
+        col = E.quantize(pred, 8)                                               # (p * 255).astype(uint8)
+        col = col[:, 0] if one_ch else np.transpose(col, (0, 2, 3, 1))
+    colored = [Image.fromarray(c) for c in col]
+    pred_np = pred.cpu().numpy()
+    pred_np = pred_np.squeeze() if not batched else (pred_np[:, 0] if one_ch else pred_np)
+    if batched:
+        if pred_np.ndim == 4 and pred_np.shape[1] == 3:
+            pred_np = np.transpose(pred_np, (0, 2, 3, 1))
+        return GenPerceptOutput(pred_np=pred_np, pred_colored=colored)
+    if pred_np.ndim == 3 and pred_np.shape[0] == 3:
+        pred_np = np.transpose(pred_np, (1, 2, 0))
+    return GenPerceptOutput(pred_np=pred_np, pred_colored=colored[0])

@@ -173,6 +173,17 @@ def remap_legacy_vae_keys(sd):
     return out
 
 
+def encoder_state(vae_sd):
+    """The VAE's encode side (encoder.*, quant_conv.*: everything encode_rgb reads) of a diffusers-layout state dict:
+    the same tensors, not copies."""
+    return {k: v for k, v in vae_sd.items() if k.startswith(("encoder.", "quant_conv."))}
+
+
+def synth_unet(seed, in_channels=4):
+    """A seeded synthetic UNet alone (the gains of ``synth_state``): task engines that share one VAE."""
+    return _synth(unet_spec(in_channels=in_channels), torch.Generator().manual_seed(seed), gain=1.0, out_gain={"conv_out": 2.0})
+
+
 def _synth(spec, gen, gain=1.0, out_gain=None):
     sd = OrderedDict()
     for k, (shape, kind) in spec.items():

@@ -111,6 +111,21 @@ gp_status gp_encode(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_hos
  * the reference always does (0: the latent already went through it, e.g. the engine's own "z").  out_dev: fp32
  * [B,C,8h,8w] in [0,1] (the reference clips to [-1,1] right after decode_pred, :470; map = out * 2 - 1). */
 gp_status gp_decode(gp_engine* e, const float* latent_dev, int apply_post_quant, float* out_dev, int out_channels, void* stream);
+/* replaces: encode_rgb for a hand-off to gp_infer_latent: the latent exactly as the plan holds it.  16-bit modes: fp32
+ * [B,4,H/8,W/8], the same as gp_encode.  High-precision mode (gp_config.precision = 1): fp32 [B,8,H/8,W/8] = [hi 0..3 |
+ * lo 0..3], the (hi, lo) fp16 pair of every value.  gp_encode's fp32 hi + lo does not determine the pair: where lo
+ * rounded to half an ulp of hi, splitting the sum again ties to even and can pick the other neighbour. */
+gp_status gp_encode_exact(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, float* latent_dev, void* stream);
+/* replaces: single_infer from rgb_latent on (genpercept_pipeline.py:411-486) for a latent gp_encode_exact produced, on this
+ * or on another engine with the same dtype, precision and VAE encoder (several task engines share one encode).
+ * latent_dev: [batch, channels, height, width] on the device as gp_encode_exact writes it (channels 4, or 8 in the
+ * high-precision mode); it must match the current plan's "rgb_latent": gp_plan(B,H,W) for the image it came from (the
+ * latent's extent alone does not fix the image's, which sets the DPT readout's and the result's extent), else
+ * GP_ERR_INVALID.  Runs the plan's UNet and readout ops (GP_STAGE_UNET .. GP_STAGE_READOUT), with their own CUDA graph
+ * when the plan uses graphs; gp_infer's graph is left as it is.  The maps equal gp_infer's on the same image bit for bit.
+ * out, out_on_host, out_channels: as gp_infer.  One-step arch only (gp_config.arch = 0; else GP_ERR_INVALID). */
+gp_status gp_infer_latent(gp_engine* e, const float* latent_dev, int batch, int channels, int height, int width, float* out,
+                          int out_on_host, int out_channels, void* stream);
 
 /* replaces: single_infer for the multi-step archs (/root/reference/genpercept/genpercept_pipeline.py:399-472; gp_config.arch = 1):
  *   rgb_latent = encode_rgb(rgb); pred_latent = noise (marigold; fp32 [B,4,h,w], host or device) or rgb_latent (noise == NULL:
