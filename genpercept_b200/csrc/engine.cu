@@ -20,31 +20,36 @@ namespace {
 const int kUnetOut[4] = {320, 640, 1280, 1280};
 const int kUnetHeads[4] = {5, 10, 20, 20};
 
-struct Kept {
-  T4 t;                 // 16-bit NHWC tensor ...
-  float* f32 = nullptr; // ... or fp32 NCHW buffer [N, C, H, W]
-  int creal = 0;        // channels exposed through read/write
-};
+bool is_set(const T4& t) { return t.off >= 0; }
 
 struct Plan {
   int B = 0, H = 0, W = 0;
   uint8_t* arena = nullptr;
   size_t arena_bytes = 0;
   std::vector<Op> ops;
-  std::map<std::string, Kept> kept;
+  // Arena tensors the entry points address.  A plan lacks (!is_set) z with the DPT readout, feat with the VAE readout
+  // and xin .. x0 on the one-step arch.
+  T4 rgb, rgb_latent, z, xin, sample, noise_pred, x0, feat[4];
   void* in_staging = nullptr;       // raw user input copy [B,3,H,W] (<= 4 bytes/elt), host inputs only
   float* out_f32 = nullptr;         // [B,3,outH,outW]: the plan's own result buffer (graph replay, host outputs, stage runs)
   float* out_dst = nullptr;         // where the final kernels write THIS launch (the caller's device buffer or out_f32);
                                     // read by the ops at launch time through Builder::out_slot
   int outH = 0, outW = 0;           // result extent: 8 * floor(H/8) (VAE readout), 64 * ceil-pyramid (DPT readout)
   uint64_t last_used = 0;
-  std::map<int, cudaGraphExec_t> graphs;   // by out_channels
+  // by (first stage, out_channels): gp_infer's and gp_infer_latent's ranges each have their own graphs and, per first
+  // stage, their own first pass, which runs eagerly (kernel attributes, lazy init)
+  std::map<std::pair<int, int>, cudaGraphExec_t> graphs;
+  std::map<int, int> eager_runs;
   double igemm_flops = 0;
-  int eager_runs = 0;                       // the first pass runs eagerly (kernel attributes, lazy init), then graphs
-  // gp_infer_latent's UNet -> readout range: its own graphs and first eager pass, so the full pipeline's stay as they are
-  std::map<int, cudaGraphExec_t> latent_graphs;
-  int latent_eager_runs = 0;
   int64_t launches = 0;
+
+  Plan() = default;
+  Plan(const Plan&) = delete;
+  Plan& operator=(const Plan&) = delete;
+  ~Plan() {
+    for (auto& g : graphs) cudaGraphExecDestroy(g.second);
+    if (arena) cudaFree(arena);
+  }
 };
 
 }  // namespace
@@ -61,12 +66,9 @@ struct gp_engine {
   Plan* cur = nullptr;
   bool mem_efficient_attn = false;   // gp_set_memory_efficient_attention: fused attention in the high-precision mode
 
-  // Synchronises, then destroys a cached plan's graph execs and frees its arena.
+  // Synchronises, then drops a cached plan (its graph execs and arena go with it).
   void drop_plan(std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>>::iterator it) {
     GP_CUDA(cudaDeviceSynchronize());
-    for (auto& g : it->second->graphs) cudaGraphExecDestroy(g.second);
-    for (auto& g : it->second->latent_graphs) cudaGraphExecDestroy(g.second);
-    if (it->second->arena) cudaFree(it->second->arena);
     if (cur == it->second.get()) cur = nullptr;
     plans.erase(it);
   }
@@ -537,17 +539,17 @@ struct gp_engine {
     GP_REQUIRE(oh <= H + 64 && ow <= W + 64, "result extent exceeds the plan's output buffer");
     if (!b.measuring()) {
       plan->outH = oh; plan->outW = ow;
-      plan->kept["rgb"] = Kept{rgb8, nullptr, 3};
-      plan->kept["rgb_latent"] = Kept{latent, nullptr, 4};
-      if (!dpt) plan->kept["z"] = Kept{z, nullptr, 4};
+      plan->rgb = rgb8;
+      plan->rgb_latent = latent;
+      if (!dpt) plan->z = z;
       if (multistep) {
-        plan->kept["xin"] = Kept{xin, nullptr, 8};
-        plan->kept["sample"] = Kept{sample, nullptr, 4};
-        plan->kept["noise_pred"] = Kept{npred, nullptr, 4};
-        plan->kept["x0"] = Kept{x0, nullptr, 4};
+        plan->xin = xin;
+        plan->sample = sample;
+        plan->noise_pred = npred;
+        plan->x0 = x0;
       }
       if (dpt)
-        for (int i = 0; i < 4; ++i) plan->kept["feat" + std::to_string(i)] = Kept{feats[i], nullptr, feats[i].C};
+        for (int i = 0; i < 4; ++i) plan->feat[i] = feats[i];
     }
   }
 };
@@ -582,6 +584,26 @@ cudaError_t run_ops(Plan* p, int stage_lo, int stage_hi, int out_channels, cudaS
   return cudaSuccess;
 }
 
+// The plan the run and inspection entry points work on; `fn` names the entry point in the error.
+Plan* current_plan(gp_engine* e, const char* fn) {
+  if (!e->cur) throw GpError(GP_ERR_NO_PLAN, std::string(fn) + ": no plan (call gp_plan)");
+  return e->cur;
+}
+
+// Points the plan's final kernels at `dst` (the caller's device buffer or out_f32) for one run, and back at out_f32 when
+// it leaves scope, on a throw too.
+struct ResultTo {
+  Plan* p;
+  ResultTo(Plan* plan, float* dst) : p(plan) { p->out_dst = dst; }
+  ~ResultTo() { p->out_dst = p->out_f32; }
+  // Copies the result to the caller's `out` when the kernels wrote it to out_f32.
+  void deliver(float* out, int out_on_host, int out_channels, cudaStream_t s) const {
+    if (p->out_dst != out)
+      GP_CUDA(cudaMemcpyAsync(out, p->out_f32, (size_t)p->B * p->outH * p->outW * out_channels * 4,
+                              out_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, s));
+  }
+};
+
 // The caller's rgb (u8, f16 or f32) -> the plan's K-packed input.  A device input is read where it lies; only host inputs
 // go through the plan's staging buffer.  `fn` names the entry point in the error message.
 void stage_rgb(gp_engine* e, Plan* p, const void* rgb, int rgb_dtype, int rgb_on_host, cudaStream_t s, const char* fn) {
@@ -596,24 +618,24 @@ void stage_rgb(gp_engine* e, Plan* p, const void* rgb, int rgb_dtype, int rgb_on
     GP_CUDA(cudaMemcpyAsync(p->in_staging, rgb, (size_t)p->B * p->H * p->W * 3 * esz, cudaMemcpyHostToDevice, s));
     src = p->in_staging;
   }
-  GP_CUDA(preprocess_rgb_im2col(src, kind, p->arena + p->kept["rgb"].t.off, p->B, p->H, p->W, e->ws.bf16, s, e->ws.split));
+  GP_CUDA(preprocess_rgb_im2col(src, kind, p->arena + p->rgb.off, p->B, p->H, p->W, e->ws.bf16, s, e->ws.split));
 }
 
 // Runs the ops of stages `first` .. GP_STAGE_READOUT and delivers the result to `out` (device, or host if out_on_host).
-// The first pass through an entry point runs eagerly (`eager_runs`); with CUDA graphs on, later passes replay the graph
-// captured in `graphs` for out_channels.
-void run_to_out(gp_engine* e, Plan* p, int first, std::map<int, cudaGraphExec_t>& graphs, int& eager_runs, float* out,
-                int out_on_host, int out_channels, cudaStream_t s) {
-  const size_t npix_out = (size_t)p->B * p->outH * p->outW;
+// The first pass from `first` runs eagerly; with CUDA graphs on, later passes replay the graph captured for
+// (first, out_channels).
+void run_to_out(gp_engine* e, Plan* p, int first, float* out, int out_on_host, int out_channels, cudaStream_t s) {
   // 2 = auto: replay a graph where the launch stream is the bottleneck — small plans
   const bool use_graph = e->cfg.use_cuda_graph == 1 ||
                          (e->cfg.use_cuda_graph == 2 && (long long)p->B * p->H * p->W <= 2LL * 768 * 768);
   // eager launches write the result straight into a device `out`; a captured graph has the plan's own buffer baked in
+  int& eager_runs = p->eager_runs[first];
   const bool graph_now = use_graph && eager_runs > 0;
-  p->out_dst = (graph_now || out_on_host) ? p->out_f32 : out;
+  ResultTo result(p, (graph_now || out_on_host) ? p->out_f32 : out);
   if (graph_now) {
-    auto it = graphs.find(out_channels);
-    if (it == graphs.end()) {
+    const auto key = std::make_pair(first, out_channels);
+    auto it = p->graphs.find(key);
+    if (it == p->graphs.end()) {
       cudaStream_t cs;
       GP_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
       cudaGraph_t g;
@@ -626,16 +648,45 @@ void run_to_out(gp_engine* e, Plan* p, int first, std::map<int, cudaGraphExec_t>
       cudaGraphExec_t ge;
       GP_CUDA(cudaGraphInstantiate(&ge, g, 0));
       cudaGraphDestroy(g);
-      it = graphs.emplace(out_channels, ge).first;
+      it = p->graphs.emplace(key, ge).first;
     }
     GP_CUDA(cudaGraphLaunch(it->second, s));
   } else {
     GP_CUDA(run_ops(p, first, GP_STAGE_READOUT, out_channels, s));
     eager_runs++;
   }
-  if (p->out_dst != out)
-    GP_CUDA(cudaMemcpyAsync(out, p->out_f32, npix_out * out_channels * 4, out_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, s));
-  p->out_dst = p->out_f32;
+  result.deliver(out, out_on_host, out_channels, s);
+}
+
+// gp_encode and gp_encode_exact: the VAE encoder on the caller's rgb; the latent leaves as fp32 [B,4,h,w], or with
+// `pair` as the high-precision mode's (hi, lo) pair, fp32 [B,8,h,w].
+gp_status encode(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, float* latent_dev, void* stream, bool pair) {
+  return guarded(e, [&]() {
+    const char* fn = pair ? "gp_encode_exact" : "gp_encode";
+    Plan* p = current_plan(e, fn);
+    GP_REQUIRE(rgb && latent_dev, std::string(fn) + ": bad arguments");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, fn);
+    GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, 1, s));
+    const T4& l = p->rgb_latent;
+    if (pair) GP_CUDA(latent_pair_to_nchw(p->arena + l.off, latent_dev, l.N, l.H, l.W, e->ws.bf16, s));
+    else GP_CUDA(nhwc8_to_nchw_f32(p->arena + l.off, latent_dev, l.N, l.H, l.W, 4, e->ws.bf16, s, e->ws.split));
+    if (rgb_on_host) GP_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+// The arena tensor gp_tensor_shape / gp_read_tensor / gp_write_tensor name, and the channels they expose.
+const T4& named_tensor(const Plan* p, const char* name, int* creal) {
+  const std::map<std::string, std::pair<const T4*, int>> named = {
+      {"rgb", {&p->rgb, 3}}, {"rgb_latent", {&p->rgb_latent, 4}}, {"z", {&p->z, 4}}, {"xin", {&p->xin, 8}},
+      {"sample", {&p->sample, 4}}, {"noise_pred", {&p->noise_pred, 4}}, {"x0", {&p->x0, 4}},
+      {"feat0", {&p->feat[0], p->feat[0].C}}, {"feat1", {&p->feat[1], p->feat[1].C}},
+      {"feat2", {&p->feat[2], p->feat[2].C}}, {"feat3", {&p->feat[3], p->feat[3].C}}};
+  auto it = named.find(name);
+  GP_REQUIRE(it != named.end() && is_set(*it->second.first), std::string("unknown tensor ") + name);
+  *creal = it->second.second;
+  return *it->second.first;
 }
 
 }  // namespace
@@ -663,15 +714,7 @@ gp_status gp_create(const gp_config* cfg, gp_engine** out) {
   return GP_OK;
 }
 
-void gp_destroy(gp_engine* e) {
-  if (!e) return;
-  for (auto& kv : e->plans) {
-    for (auto& g : kv.second->graphs) cudaGraphExecDestroy(g.second);
-    for (auto& g : kv.second->latent_graphs) cudaGraphExecDestroy(g.second);
-    if (kv.second->arena) cudaFree(kv.second->arena);
-  }
-  delete e;
-}
+void gp_destroy(gp_engine* e) { delete e; }
 
 const char* gp_last_error(gp_engine* e) { return e ? e->err.c_str() : "null engine"; }
 
@@ -721,6 +764,7 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
     GP_CUDA(cudaSetDevice(e->cfg.device));
     auto key = std::make_tuple(B, H, W);
     auto it = e->plans.find(key);
+    // Only gp_plan stamps a plan: it is also the only place `cur` changes, so the current plan is always the newest.
     if (it != e->plans.end()) { e->cur = it->second.get(); e->cur->last_used = ++e->use_clock; return; }
     // Bounded plan cache (a folder of in-the-wild images yields a new (H, W) per aspect ratio): evict the least
     // recently used plans — graph execs destroyed, arena freed — before building another one.
@@ -741,7 +785,6 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
     if (ae == cudaErrorMemoryAllocation) {
       // Not a sticky error: clear it and report the shape as too large, so the engine stays usable for smaller inputs.
       cudaGetLastError();
-      p->arena = nullptr;
       throw GpError(GP_ERR_INVALID, "gp_plan: batch " + std::to_string(B) + " at " + std::to_string(H) + "x" +
                                         std::to_string(W) + " needs an activation arena of " +
                                         std::to_string(p->arena_bytes) + " bytes, more than the device can allocate");
@@ -750,7 +793,6 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
     if (!m.long_softmax.empty()) {
       // The arena fits, but the unfused softmax of this attention cannot run: fail here, not with a CUDA error at
       // inference, and leave the engine usable.
-      cudaFree(p->arena);
       throw GpError(GP_ERR_INVALID, "gp_plan: batch " + std::to_string(B) + " at " + std::to_string(H) + "x" +
                                         std::to_string(W) + ": " + m.long_softmax + " has rows past " +
                                         std::to_string(kSoftmaxRowsMaxT) + " keys, more than the unfused softmax takes; "
@@ -802,17 +844,14 @@ gp_status gp_set_timestep(gp_engine* e, int timestep) {
 gp_status gp_infer(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, float* out, int out_on_host,
                    int out_channels, void* stream) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_infer: no plan (call gp_plan)");
+    Plan* p = current_plan(e, "gp_infer");
     if (e->multistep) throw GpError(GP_ERR_STATE, "gp_infer: this engine runs the multi-step arch (gp_infer_steps)");
-    const bool dpt = e->cfg.readout == GP_READOUT_DPT;
-    if (dpt) out_channels = 1;
+    if (e->cfg.readout == GP_READOUT_DPT) out_channels = 1;
     GP_REQUIRE(rgb && out && (out_channels == 1 || out_channels == 3), "gp_infer: bad arguments");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
-    p->last_used = ++e->use_clock;
     stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_infer");
-    run_to_out(e, p, GP_STAGE_VAE_ENCODE, p->graphs, p->eager_runs, out, out_on_host, out_channels, s);
+    run_to_out(e, p, GP_STAGE_VAE_ENCODE, out, out_on_host, out_channels, s);
     if (rgb_on_host || out_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }
@@ -821,11 +860,10 @@ gp_status gp_infer_latent(gp_engine* e, const float* latent_dev, int batch, int 
                           int out_on_host, int out_channels, void* stream) {
   return guarded(e, [&]() {
     if (e->multistep) throw GpError(GP_ERR_INVALID, "gp_infer_latent: runs the one-step arch only (gp_config.arch = 0)");
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_infer_latent: no plan (call gp_plan)");
+    Plan* p = current_plan(e, "gp_infer_latent");
     if (e->cfg.readout == GP_READOUT_DPT) out_channels = 1;
     GP_REQUIRE(latent_dev && out && (out_channels == 1 || out_channels == 3), "gp_infer_latent: bad arguments");
-    const T4& lat = p->kept["rgb_latent"].t;
+    const T4& lat = p->rgb_latent;
     const int lat_c = e->ws.split ? 8 : 4;
     GP_REQUIRE(batch == lat.N && channels == lat_c && height == lat.H && width == lat.W,
                "gp_infer_latent: latent [" + std::to_string(batch) + "," + std::to_string(channels) + "," + std::to_string(height) +
@@ -834,60 +872,34 @@ gp_status gp_infer_latent(gp_engine* e, const float* latent_dev, int batch, int 
                    (e->ws.split ? " (the high-precision mode takes the (hi, lo) pair gp_encode_exact writes)" : ""));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
-    p->last_used = ++e->use_clock;
     if (e->ws.split) GP_CUDA(latent_pair_from_nchw(latent_dev, p->arena + lat.off, lat.N, lat.H, lat.W, e->ws.bf16, s));
     else GP_CUDA(nchw4_affine_to_nhwc8(latent_dev, p->arena + lat.off, lat.N, lat.H, lat.W, 1.0f, nullptr, nullptr, e->ws.bf16, s));
-    run_to_out(e, p, GP_STAGE_UNET, p->latent_graphs, p->latent_eager_runs, out, out_on_host, out_channels, s);
+    run_to_out(e, p, GP_STAGE_UNET, out, out_on_host, out_channels, s);
     if (out_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }
 
 gp_status gp_encode(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, float* latent_dev, void* stream) {
-  return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_encode: no plan (call gp_plan)");
-    GP_REQUIRE(rgb && latent_dev, "gp_encode: bad arguments");
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    GP_CUDA(cudaSetDevice(e->cfg.device));
-    stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_encode");
-    GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, 1, s));
-    const T4& l = p->kept["rgb_latent"].t;
-    GP_CUDA(nhwc8_to_nchw_f32(p->arena + l.off, latent_dev, l.N, l.H, l.W, 4, e->ws.bf16, s, e->ws.split));
-    if (rgb_on_host) GP_CUDA(cudaStreamSynchronize(s));
-  });
+  return encode(e, rgb, rgb_dtype, rgb_on_host, latent_dev, stream, false);
 }
 
 gp_status gp_encode_exact(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, float* latent_dev, void* stream) {
-  if (e && !e->ws.split) return gp_encode(e, rgb, rgb_dtype, rgb_on_host, latent_dev, stream);
-  return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_encode_exact: no plan (call gp_plan)");
-    GP_REQUIRE(rgb && latent_dev, "gp_encode_exact: bad arguments");
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    GP_CUDA(cudaSetDevice(e->cfg.device));
-    stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_encode_exact");
-    GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, 1, s));
-    const T4& l = p->kept["rgb_latent"].t;
-    GP_CUDA(latent_pair_to_nchw(p->arena + l.off, latent_dev, l.N, l.H, l.W, e->ws.bf16, s));
-    if (rgb_on_host) GP_CUDA(cudaStreamSynchronize(s));
-  });
+  return encode(e, rgb, rgb_dtype, rgb_on_host, latent_dev, stream, e && e->ws.split);
 }
 
 gp_status gp_decode(gp_engine* e, const float* latent_dev, int apply_post_quant, float* out_dev, int out_channels, void* stream) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_decode: no plan (call gp_plan)");
+    Plan* p = current_plan(e, "gp_decode");
     if (e->cfg.readout == GP_READOUT_DPT) throw GpError(GP_ERR_STATE, "gp_decode: the DPT readout has no latent decoder");
     GP_REQUIRE(latent_dev && out_dev && (out_channels == 1 || out_channels == 3), "gp_decode: bad arguments");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
-    const T4& z = p->kept["z"].t;
+    const T4& z = p->z;
     GP_CUDA(nchw4_affine_to_nhwc8(latent_dev, p->arena + z.off, z.N, z.H, z.W, 1.0f / kLatentScale,
                                   apply_post_quant ? e->ws.pq_dev : nullptr, apply_post_quant ? e->ws.pq_dev + 16 : nullptr, e->ws.bf16, s,
                                   e->ws.split));
-    p->out_dst = out_dev;
+    ResultTo result(p, out_dev);
     GP_CUDA(run_ops(p, GP_STAGE_READOUT, GP_STAGE_READOUT, out_channels, s));
-    p->out_dst = p->out_f32;
   });
 }
 
@@ -895,19 +907,17 @@ gp_status gp_infer_steps(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_o
                          const int* timesteps, const float* coeffs, int n_steps, float* out, int out_on_host, int out_channels,
                          void* stream) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_infer_steps: no plan (call gp_plan)");
+    Plan* p = current_plan(e, "gp_infer_steps");
     if (!e->multistep) throw GpError(GP_ERR_STATE, "gp_infer_steps needs gp_config.arch = 1");
     GP_REQUIRE(rgb && out && timesteps && coeffs && n_steps >= 1 && (out_channels == 1 || out_channels == 3), "gp_infer_steps: bad arguments");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
-    p->last_used = ++e->use_clock;
     stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_infer_steps");
     GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, out_channels, s));      // rgb_latent (:416)
-    const T4& lat = p->kept["rgb_latent"].t;
+    const T4& lat = p->rgb_latent;
     const long long npx = lat.pixels();
     uint8_t* A = p->arena;
-    void* smp = A + p->kept["sample"].t.off;
+    void* smp = A + p->sample.off;
     if (noise) {              // marigold: pred_latent = randn (:418-425; the caller draws it with its generator)
       const float* nd = noise;
       if (noise_on_host) {    // the plan's result buffer is free until the decoder runs
@@ -919,49 +929,44 @@ gp_status gp_infer_steps(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_o
       GP_CUDA(cudaMemcpyAsync(smp, A + lat.off, lat.bytes(), cudaMemcpyDeviceToDevice, s));
     }
     for (int i = 0; i < n_steps; ++i) {                                                  // :443-463
-      GP_CUDA(latent_pack(A + lat.off, smp, A + p->kept["xin"].t.off, npx, e->unet_in_ch, e->ws.bf16, s, e->ws.split));
+      GP_CUDA(latent_pack(A + lat.off, smp, A + p->xin.off, npx, e->unet_in_ch, e->ws.bf16, s, e->ws.split));
       e->ws.set_timestep(timesteps[i]);
       GP_CUDA(run_ops(p, GP_STAGE_UNET, GP_STAGE_UNET, out_channels, s));
-      GP_CUDA(ddim_step(A + p->kept["noise_pred"].t.off, smp, A + p->kept["x0"].t.off, npx, coeffs + 4 * i, e->ws.bf16, s, e->ws.split));
+      GP_CUDA(ddim_step(A + p->noise_pred.off, smp, A + p->x0.off, npx, coeffs + 4 * i, e->ws.bf16, s, e->ws.split));
     }
     // pred_latent = step_output.pred_original_sample (:465); decode_pred (:507-526); clip + shift in the last kernel
-    GP_CUDA(latent_affine(A + p->kept["x0"].t.off, A + p->kept["z"].t.off, npx, 1.0f / kLatentScale, e->ws.pq_dev, e->ws.pq_dev + 16,
+    GP_CUDA(latent_affine(A + p->x0.off, A + p->z.off, npx, 1.0f / kLatentScale, e->ws.pq_dev, e->ws.pq_dev + 16,
                           e->ws.bf16, s, e->ws.split));
-    p->out_dst = out_on_host ? p->out_f32 : out;
+    ResultTo result(p, out_on_host ? p->out_f32 : out);
     GP_CUDA(run_ops(p, GP_STAGE_READOUT, GP_STAGE_READOUT, out_channels, s));
-    if (p->out_dst != out)
-      GP_CUDA(cudaMemcpyAsync(out, p->out_f32, (size_t)p->B * p->outH * p->outW * out_channels * 4, cudaMemcpyDeviceToHost, s));
-    p->out_dst = p->out_f32;
+    result.deliver(out, out_on_host, out_channels, s);
     if (rgb_on_host || out_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }
 
 gp_status gp_run_stage(gp_engine* e, int stage, int out_channels, void* stream) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "gp_run_stage: no plan");
+    Plan* p = current_plan(e, "gp_run_stage");
     if (e->cfg.readout == GP_READOUT_DPT) out_channels = 1;
     GP_CUDA(cudaSetDevice(e->cfg.device));
-    p->out_dst = p->out_f32;
+    ResultTo result(p, p->out_f32);
     GP_CUDA(run_ops(p, stage, stage, out_channels, reinterpret_cast<cudaStream_t>(stream)));
   });
 }
 
 gp_status gp_tensor_shape(gp_engine* e, const char* name, int64_t shape[4]) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "no plan");
+    Plan* p = current_plan(e, "gp_tensor_shape");
     if (std::string(name) == "out") { shape[0] = p->B; shape[1] = 3; shape[2] = p->outH; shape[3] = p->outW; return; }
-    auto it = p->kept.find(name);
-    GP_REQUIRE(it != p->kept.end(), std::string("unknown tensor ") + name);
-    shape[0] = it->second.t.N; shape[1] = it->second.creal; shape[2] = it->second.t.H; shape[3] = it->second.t.W;
+    int cr = 0;
+    const T4& t = named_tensor(p, name, &cr);
+    shape[0] = t.N; shape[1] = cr; shape[2] = t.H; shape[3] = t.W;
   });
 }
 
 gp_status gp_read_tensor(gp_engine* e, const char* name, float* host_out, size_t cap) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "no plan");
+    Plan* p = current_plan(e, "gp_read_tensor");
     GP_CUDA(cudaDeviceSynchronize());
     if (std::string(name) == "out") {
       const size_t n = (size_t)p->B * 3 * p->outH * p->outW;
@@ -969,10 +974,8 @@ gp_status gp_read_tensor(gp_engine* e, const char* name, float* host_out, size_t
       GP_CUDA(cudaMemcpy(host_out, p->out_f32, n * 4, cudaMemcpyDeviceToHost));
       return;
     }
-    auto it = p->kept.find(name);
-    GP_REQUIRE(it != p->kept.end(), std::string("unknown tensor ") + name);
-    const T4& t = it->second.t;
-    const int cr = it->second.creal;
+    int cr = 0;
+    const T4& t = named_tensor(p, name, &cr);
     GP_REQUIRE(cap >= (size_t)t.N * cr * t.H * t.W, "gp_read_tensor: buffer too small");
     const size_t ps = (size_t)t.ps();
     std::vector<uint16_t> h((size_t)t.N * t.H * t.W * ps);
@@ -989,12 +992,9 @@ gp_status gp_read_tensor(gp_engine* e, const char* name, float* host_out, size_t
 
 gp_status gp_write_tensor(gp_engine* e, const char* name, const float* host_in, size_t elems) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "no plan");
-    auto it = p->kept.find(name);
-    GP_REQUIRE(it != p->kept.end(), std::string("unknown tensor ") + name);
-    const T4& t = it->second.t;
-    const int cr = it->second.creal;
+    Plan* p = current_plan(e, "gp_write_tensor");
+    int cr = 0;
+    const T4& t = named_tensor(p, name, &cr);
     GP_REQUIRE(elems == (size_t)t.N * cr * t.H * t.W, "gp_write_tensor: size mismatch");
     const size_t ps = (size_t)t.ps();
     std::vector<uint16_t> h((size_t)t.N * t.H * t.W * ps, 0);
@@ -1015,8 +1015,7 @@ gp_status gp_write_tensor(gp_engine* e, const char* name, const float* host_in, 
 gp_status gp_plan_info(gp_engine* e, int64_t* n_ops, int64_t* n_launches, int64_t* arena_bytes, int64_t* weight_bytes,
                        double* igemm_flops) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "no plan");
+    Plan* p = current_plan(e, "gp_plan_info");
     if (n_ops) *n_ops = (int64_t)p->ops.size();
     if (n_launches) *n_launches = p->launches + 1;   // + preprocess
     if (arena_bytes) *arena_bytes = (int64_t)p->arena_bytes;
@@ -1027,14 +1026,13 @@ gp_status gp_plan_info(gp_engine* e, int64_t* n_ops, int64_t* n_launches, int64_
 
 gp_status gp_profile_ops(gp_engine* e, int out_channels, void* stream) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "no plan");
+    Plan* p = current_plan(e, "gp_profile_ops");
     if (e->cfg.readout == GP_READOUT_DPT) out_channels = 1;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     cudaEvent_t a, b;
     GP_CUDA(cudaEventCreate(&a));
     GP_CUDA(cudaEventCreate(&b));
-    p->out_dst = p->out_f32;
+    ResultTo result(p, p->out_f32);
     for (auto& op : p->ops) {
       op.usec = 0;
       if (op.variant != 0 && op.variant != out_channels) continue;
@@ -1054,8 +1052,7 @@ gp_status gp_profile_ops(gp_engine* e, int out_channels, void* stream) {
 gp_status gp_op_info(gp_engine* e, int64_t i, char* name_buf, size_t name_cap, double* usec, double* flops, double* bytes,
                      int* kind, double* flops_exec) {
   return guarded(e, [&]() {
-    Plan* p = e->cur;
-    if (!p) throw GpError(GP_ERR_NO_PLAN, "no plan");
+    Plan* p = current_plan(e, "gp_op_info");
     GP_REQUIRE(i >= 0 && i < (int64_t)p->ops.size(), "op index out of range");
     const Op& op = p->ops[(size_t)i];
     if (name_buf && name_cap) { std::strncpy(name_buf, op.name.c_str(), name_cap - 1); name_buf[name_cap - 1] = 0; }

@@ -60,6 +60,22 @@ double time_ops(Builder& b, int iters) {
   return ms * 1000.0 / iters;
 }
 
+// Fills the attention benchmarks' 16-bit operands `qk` (qk_n elements) and `vT` (vt_n) with small pseudo-random values
+// (scores of order one, as in the model) rather than zeros, so the tensor cores switch as they do on real data.
+void fill_attention_operands(bool bf16, void* qk, size_t qk_n, void* vT, size_t vt_n) {
+  std::vector<uint16_t> pat((size_t)1 << 20);
+  uint32_t x = 12345u;
+  for (auto& v : pat) {
+    x = x * 1664525u + 1013904223u;
+    const float f = ((int)(x >> 9) - (1 << 22)) * (0.3f / (1 << 22));
+    v = host_f2h(f, bf16);
+  }
+  for (auto [buf, n] : {std::make_pair(qk, qk_n), std::make_pair(vT, vt_n)})
+    for (size_t i = 0; i < n; i += pat.size())
+      GP_CUDA(cudaMemcpy(reinterpret_cast<uint16_t*>(buf) + i, pat.data(), std::min(pat.size(), n - i) * 2,
+                         cudaMemcpyHostToDevice));
+}
+
 }  // namespace
 
 extern "C" {
@@ -291,21 +307,7 @@ gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, doub
     void* qk = ws.device_alloc(qk_n * 2);
     void* vT = ws.device_alloc(vt_n * 2);
     void* o = ws.device_alloc(o_n * 2);
-    // Small pseudo-random operands (scores of order one, as in the model) rather than zeros, so the tensor cores switch
-    // as they do on real data.
-    {
-      std::vector<uint16_t> pat((size_t)1 << 20);
-      uint32_t x = 12345u;
-      for (auto& v : pat) {
-        x = x * 1664525u + 1013904223u;
-        const float f = ((int)(x >> 9) - (1 << 22)) * (0.3f / (1 << 22));
-        v = host_f2h(f, ws.bf16);
-      }
-      for (auto [buf, n] : {std::make_pair(qk, qk_n), std::make_pair(vT, vt_n)})
-        for (size_t i = 0; i < n; i += pat.size())
-          GP_CUDA(cudaMemcpy(reinterpret_cast<uint16_t*>(buf) + i, pat.data(), std::min(pat.size(), n - i) * 2,
-                             cudaMemcpyHostToDevice));
-    }
+    fill_attention_operands(ws.bf16, qk, qk_n, vT, vt_n);
     // one warm-up launch, synchronised
     Builder b = build_and_run(ws, 0, [&](Builder& bb) {
       bb.attn512_path = fused ? 1 : 0;
@@ -330,20 +332,7 @@ gp_status gp_bench_attention_high(int B, int T, int heads, int d, int fused, int
     void* qk = ws.device_alloc(qk_n * 2);
     void* vT = ws.device_alloc(vt_n * 2);
     void* o = ws.device_alloc(o_n * 2);
-    // small pseudo-random operands (scores of order one), lo planes included, so the tensor cores switch as on real data
-    {
-      std::vector<uint16_t> pat((size_t)1 << 20);
-      uint32_t x = 12345u;
-      for (auto& v : pat) {
-        x = x * 1664525u + 1013904223u;
-        const float f = ((int)(x >> 9) - (1 << 22)) * (0.3f / (1 << 22));
-        v = host_f2h(f, false);
-      }
-      for (auto [buf, n] : {std::make_pair(qk, qk_n), std::make_pair(vT, vt_n)})
-        for (size_t i = 0; i < n; i += pat.size())
-          GP_CUDA(cudaMemcpy(reinterpret_cast<uint16_t*>(buf) + i, pat.data(), std::min(pat.size(), n - i) * 2,
-                             cudaMemcpyHostToDevice));
-    }
+    fill_attention_operands(false, qk, qk_n, vT, vt_n);     // lo planes included
     // one warm-up launch, synchronised
     Builder b = build_and_run(ws, 0, [&](Builder& bb) {
       bb.mem_efficient_attn = fused != 0;

@@ -105,6 +105,16 @@ def _stream_ptr(device=None):
     return c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def _on_host(t):
+    """The C-ABI's on-host flag of a buffer."""
+    return 0 if t.is_cuda else 1
+
+
+def _rgb_arg(rgb):
+    """An rgb batch as the C-ABI takes it: contiguous, with bf16 (which it does not take) as fp32."""
+    return (rgb.float() if rgb.dtype == torch.bfloat16 else rgb).contiguous()
+
+
 def _check_free(st, what):
     if st != 0:
         raise RuntimeError(f"{what} failed: {_STATUS.get(st, st)} (see stderr)")
@@ -194,14 +204,26 @@ class Engine:
     def _sp(self):
         return _stream_ptr(self.device)
 
+    def _plan_for(self, B, H, W):
+        if self.plan_shape != (B, H, W):
+            self.plan(B, H, W)
+
+    def _out(self, out, B, C):
+        """The caller's `out`, checked, or a new device buffer: contiguous fp32 [B, C, *out_hw]."""
+        shape = (B, C) + tuple(self.out_hw or (0, 0))      # no plan (infer_latent): the library reports GP_ERR_NO_PLAN
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32, device=self.device)
+        assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == shape, \
+            f"out must be contiguous fp32 {shape}"
+        return out
+
     def encode(self, rgb):
         """encode_rgb on the device: [B,3,H,W] uint8 / float -> fp32 latent [B,4,H/8,W/8] (cuda)."""
         B, _, H, W = rgb.shape
-        if self.plan_shape != (B, H, W):
-            self.plan(B, H, W)
-        rgb = (rgb.float() if rgb.dtype == torch.bfloat16 else rgb).contiguous()
+        self._plan_for(B, H, W)
+        rgb = _rgb_arg(rgb)
         lat = torch.empty((B, 4) + self.tensor_shape("rgb_latent")[2:], dtype=torch.float32, device=self.device)
-        self._ck(self.L.gp_encode(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), 0 if rgb.is_cuda else 1,
+        self._ck(self.L.gp_encode(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), _on_host(rgb),
                                   c_void_p(lat.data_ptr()), self._sp()), "gp_encode")
         return lat
 
@@ -221,19 +243,12 @@ class Engine:
         Returns fp32 [B,C,H,W] in [0,1] on the device of `out` (default: cuda)."""
         assert rgb.dim() == 4 and rgb.shape[1] == 3
         B, _, H, W = rgb.shape
-        if self.plan_shape != (B, H, W):
-            self.plan(B, H, W)
-        if rgb.dtype == torch.bfloat16:
-            rgb = rgb.float()
-        rgb = rgb.contiguous()
+        self._plan_for(B, H, W)
+        rgb = _rgb_arg(rgb)
         C = 1 if self.readout == "dpt" else out_channels
-        Ho, Wo = self.out_hw
-        if out is None:
-            out = torch.empty((B, C, Ho, Wo), dtype=torch.float32, device=self.device)
-        assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (B, C, Ho, Wo), \
-            f"out must be contiguous fp32 {(B, C, Ho, Wo)}"
-        self._ck(self.L.gp_infer(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), 0 if rgb.is_cuda else 1,
-                                 c_void_p(out.data_ptr()), 0 if out.is_cuda else 1, C, self._sp()), "gp_infer")
+        out = self._out(out, B, C)
+        self._ck(self.L.gp_infer(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), _on_host(rgb),
+                                 c_void_p(out.data_ptr()), _on_host(out), C, self._sp()), "gp_infer")
         return out
 
     def encode_exact(self, rgb):
@@ -241,12 +256,11 @@ class Engine:
         [B,4,H/8,W/8] (cuda) in the 16-bit modes, the same as ``encode``; in the high-precision mode fp32 [B,8,H/8,W/8] =
         [hi | lo], the (hi, lo) pair of every value.  Plans (B, H, W) like ``infer``."""
         B, _, H, W = rgb.shape
-        if self.plan_shape != (B, H, W):
-            self.plan(B, H, W)
-        rgb = (rgb.float() if rgb.dtype == torch.bfloat16 else rgb).contiguous()
+        self._plan_for(B, H, W)
+        rgb = _rgb_arg(rgb)
         c = 8 if self.precision == "high" else 4
         lat = torch.empty((B, c) + self.tensor_shape("rgb_latent")[2:], dtype=torch.float32, device=self.device)
-        self._ck(self.L.gp_encode_exact(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), 0 if rgb.is_cuda else 1,
+        self._ck(self.L.gp_encode_exact(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), _on_host(rgb),
                                         c_void_p(lat.data_ptr()), self._sp()), "gp_encode_exact")
         return lat
 
@@ -259,13 +273,9 @@ class Engine:
         B, c, h, w = latent.shape
         latent = latent.to(self.device, torch.float32).contiguous()
         C = 1 if self.readout == "dpt" else out_channels
-        Ho, Wo = self.out_hw if self.out_hw is not None else (0, 0)     # no plan: the library reports GP_ERR_NO_PLAN
-        if out is None:
-            out = torch.empty((B, C, Ho, Wo), dtype=torch.float32, device=self.device)
-        assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (B, C, Ho, Wo), \
-            f"out must be contiguous fp32 {(B, C, Ho, Wo)}"
+        out = self._out(out, B, C)
         self._ck(self.L.gp_infer_latent(self.h, c_void_p(latent.data_ptr()), B, c, h, w, c_void_p(out.data_ptr()),
-                                        0 if out.is_cuda else 1, C, self._sp()), "gp_infer_latent")
+                                        _on_host(out), C, self._sp()), "gp_infer_latent")
         return out
 
     def infer_steps(self, rgb, timesteps, coeffs, noise=None, out_channels=1, out=None):
@@ -273,12 +283,9 @@ class Engine:
         (scheduler.DDIMSchedule.step_coefficients), `noise` fp32 [B,4,h,w] (marigold) or None (rgb_blending)."""
         assert rgb.dim() == 4 and rgb.shape[1] == 3
         B, _, H, W = rgb.shape
-        if self.plan_shape != (B, H, W):
-            self.plan(B, H, W)
-        rgb = (rgb.float() if rgb.dtype == torch.bfloat16 else rgb).contiguous()
-        Ho, Wo = self.out_hw
-        if out is None:
-            out = torch.empty((B, out_channels, Ho, Wo), dtype=torch.float32, device=self.device)
+        self._plan_for(B, H, W)
+        rgb = _rgb_arg(rgb)
+        out = self._out(out, B, out_channels)
         n = len(timesteps)
         ts = (c_int * n)(*[int(t) for t in timesteps])
         cf = (c_float * (4 * n))(*[float(v) for row in coeffs for v in row])
@@ -286,9 +293,9 @@ class Engine:
         if noise is not None:
             nz = noise.detach().to(torch.float32).contiguous()
             assert tuple(nz.shape) == (B, 4) + tuple(self.tensor_shape("rgb_latent")[2:]), "noise must be [B,4,H/8,W/8]"
-        self._ck(self.L.gp_infer_steps(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), 0 if rgb.is_cuda else 1,
-                                       c_void_p(nz.data_ptr()) if nz is not None else None, 0 if (nz is None or nz.is_cuda) else 1,
-                                       ts, cf, n, c_void_p(out.data_ptr()), 0 if out.is_cuda else 1, out_channels, self._sp()),
+        self._ck(self.L.gp_infer_steps(self.h, c_void_p(rgb.data_ptr()), _gp_dtype(rgb.dtype), _on_host(rgb),
+                                       c_void_p(nz.data_ptr()) if nz is not None else None, _on_host(nz) if nz is not None else 0,
+                                       ts, cf, n, c_void_p(out.data_ptr()), _on_host(out), out_channels, self._sp()),
                  "gp_infer_steps")
         return out
 
