@@ -26,6 +26,8 @@ struct Plan {
   int B = 0, H = 0, W = 0;
   uint8_t* arena = nullptr;
   size_t arena_bytes = 0;
+  bool shared = false;              // the arena is the device's shared pool (gp_set_shared_arena), not the plan's own
+  int device = 0;
   std::vector<Op> ops;
   // Arena tensors the entry points address.  A plan lacks (!is_set) z with the DPT readout, feat with the VAE readout
   // and xin .. x0 on the one-step arch.
@@ -48,7 +50,20 @@ struct Plan {
   Plan& operator=(const Plan&) = delete;
   ~Plan() {
     for (auto& g : graphs) cudaGraphExecDestroy(g.second);
-    if (arena) cudaFree(arena);
+    if (shared) shared_arena_remove(device, arena_bytes);
+    else if (arena) cudaFree(arena);
+  }
+};
+
+// Orders one entry point's use of a shared plan's arena after every earlier user of the pool, whatever its engine or
+// stream, and before every later one: one event wait when the call starts, one record when it ends (on a throw too).
+struct ArenaUse {
+  const Plan* p;
+  cudaStream_t s;
+  ArenaUse(const Plan* plan, cudaStream_t st) : p(plan), s(st) { if (p->shared) shared_arena_wait(p->device, s); }
+  ~ArenaUse() {
+    if (!p->shared) return;
+    try { shared_arena_record(p->device, s); } catch (const GpError&) {}   // the call already reports the CUDA error
   }
 };
 
@@ -65,6 +80,14 @@ struct gp_engine {
   std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>> plans;
   Plan* cur = nullptr;
   bool mem_efficient_attn = false;   // gp_set_memory_efficient_attention: fused attention in the high-precision mode
+  bool shared_arena = false;         // gp_set_shared_arena: new plans take their arena from the device's shared pool
+
+  ~gp_engine() {
+    if (!shared_arena) return;
+    cudaSetDevice(cfg.device);
+    plans.clear();             // each shared plan gives its share back before the engine leaves the pool
+    shared_arena_leave(cfg.device);
+  }
 
   // Synchronises, then drops a cached plan (its graph execs and arena go with it).
   void drop_plan(std::map<std::tuple<int, int, int>, std::unique_ptr<Plan>>::iterator it) {
@@ -667,6 +690,7 @@ gp_status encode(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, 
     GP_REQUIRE(rgb && latent_dev, std::string(fn) + ": bad arguments");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
+    ArenaUse use(p, s);
     stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, fn);
     GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, 1, s));
     const T4& l = p->rgb_latent;
@@ -780,16 +804,23 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
     e->build(m, nullptr, B, H, W);
     std::unique_ptr<Plan> p(new Plan());
     p->B = B; p->H = H; p->W = W;
+    p->device = e->cfg.device;
     p->arena_bytes = m.arena_bytes();
-    const cudaError_t ae = cudaMalloc(reinterpret_cast<void**>(&p->arena), p->arena_bytes);
-    if (ae == cudaErrorMemoryAllocation) {
+    bool too_large = false;
+    if (e->shared_arena) {
+      p->arena = shared_arena_add(p->device, p->arena_bytes);
+      p->shared = p->arena != nullptr;
+      too_large = !p->shared;
+    } else {
+      const cudaError_t ae = cudaMalloc(reinterpret_cast<void**>(&p->arena), p->arena_bytes);
       // Not a sticky error: clear it and report the shape as too large, so the engine stays usable for smaller inputs.
-      cudaGetLastError();
+      if (ae == cudaErrorMemoryAllocation) { cudaGetLastError(); too_large = true; }
+      else GP_CUDA(ae);
+    }
+    if (too_large)
       throw GpError(GP_ERR_INVALID, "gp_plan: batch " + std::to_string(B) + " at " + std::to_string(H) + "x" +
                                         std::to_string(W) + " needs an activation arena of " +
                                         std::to_string(p->arena_bytes) + " bytes, more than the device can allocate");
-    }
-    GP_CUDA(ae);
     if (!m.long_softmax.empty()) {
       // The arena fits, but the unfused softmax of this attention cannot run: fail here, not with a CUDA error at
       // inference, and leave the engine usable.
@@ -798,7 +829,12 @@ gp_status gp_plan(gp_engine* e, int B, int H, int W) {
                                         std::to_string(kSoftmaxRowsMaxT) + " keys, more than the unfused softmax takes; "
                                         "enable memory-efficient attention (gp_set_memory_efficient_attention)");
     }
-    GP_CUDA(cudaMemset(p->arena, 0, p->arena_bytes));
+    if (p->shared) {   // on the legacy stream like cudaMemset, after the pool's earlier users on any stream
+      ArenaUse use(p.get(), nullptr);
+      GP_CUDA(cudaMemsetAsync(p->arena, 0, p->arena_bytes, nullptr));
+    } else {
+      GP_CUDA(cudaMemset(p->arena, 0, p->arena_bytes));
+    }
     Builder b(e->ws.bf16, false, p->arena, e->ws.split);
     b.mem_efficient_attn = e->mem_efficient_attn;
     e->build(b, p.get(), B, H, W);
@@ -827,6 +863,18 @@ gp_status gp_set_memory_efficient_attention(gp_engine* e, int enable) {
   });
 }
 
+gp_status gp_set_shared_arena(gp_engine* e, int enable) {
+  return guarded(e, [&]() {
+    const bool on = enable != 0;
+    if (on == e->shared_arena) return;
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    while (!e->plans.empty()) e->drop_plan(e->plans.begin());
+    if (on) shared_arena_join(e->cfg.device);
+    else shared_arena_leave(e->cfg.device);
+    e->shared_arena = on;
+  });
+}
+
 gp_status gp_tile_shape(int cout, int cin, int ks, int images, int h, int w, int tokens_mode, int num_sms, int* bn, int* mt) {
   if (!bn || !mt || cout < 1 || cin < 1 || ks < 1 || images < 1 || h < 1 || w < 1 || num_sms < 1) return GP_ERR_INVALID;
   gp::tile_shape_for(cout, (double)cin * ks * ks, tokens_mode != 0, images, w, h, num_sms, bn, mt);
@@ -850,6 +898,7 @@ gp_status gp_infer(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host
     GP_REQUIRE(rgb && out && (out_channels == 1 || out_channels == 3), "gp_infer: bad arguments");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
+    ArenaUse use(p, s);
     stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_infer");
     run_to_out(e, p, GP_STAGE_VAE_ENCODE, out, out_on_host, out_channels, s);
     if (rgb_on_host || out_on_host) GP_CUDA(cudaStreamSynchronize(s));
@@ -872,6 +921,7 @@ gp_status gp_infer_latent(gp_engine* e, const float* latent_dev, int batch, int 
                    (e->ws.split ? " (the high-precision mode takes the (hi, lo) pair gp_encode_exact writes)" : ""));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
+    ArenaUse use(p, s);
     if (e->ws.split) GP_CUDA(latent_pair_from_nchw(latent_dev, p->arena + lat.off, lat.N, lat.H, lat.W, e->ws.bf16, s));
     else GP_CUDA(nchw4_affine_to_nhwc8(latent_dev, p->arena + lat.off, lat.N, lat.H, lat.W, 1.0f, nullptr, nullptr, e->ws.bf16, s));
     run_to_out(e, p, GP_STAGE_UNET, out, out_on_host, out_channels, s);
@@ -894,6 +944,7 @@ gp_status gp_decode(gp_engine* e, const float* latent_dev, int apply_post_quant,
     GP_REQUIRE(latent_dev && out_dev && (out_channels == 1 || out_channels == 3), "gp_decode: bad arguments");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
+    ArenaUse use(p, s);
     const T4& z = p->z;
     GP_CUDA(nchw4_affine_to_nhwc8(latent_dev, p->arena + z.off, z.N, z.H, z.W, 1.0f / kLatentScale,
                                   apply_post_quant ? e->ws.pq_dev : nullptr, apply_post_quant ? e->ws.pq_dev + 16 : nullptr, e->ws.bf16, s,
@@ -912,6 +963,7 @@ gp_status gp_infer_steps(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_o
     GP_REQUIRE(rgb && out && timesteps && coeffs && n_steps >= 1 && (out_channels == 1 || out_channels == 3), "gp_infer_steps: bad arguments");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
+    ArenaUse use(p, s);
     stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_infer_steps");
     GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, out_channels, s));      // rgb_latent (:416)
     const T4& lat = p->rgb_latent;
@@ -949,8 +1001,10 @@ gp_status gp_run_stage(gp_engine* e, int stage, int out_channels, void* stream) 
     Plan* p = current_plan(e, "gp_run_stage");
     if (e->cfg.readout == GP_READOUT_DPT) out_channels = 1;
     GP_CUDA(cudaSetDevice(e->cfg.device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    ArenaUse use(p, s);
     ResultTo result(p, p->out_f32);
-    GP_CUDA(run_ops(p, stage, stage, out_channels, reinterpret_cast<cudaStream_t>(stream)));
+    GP_CUDA(run_ops(p, stage, stage, out_channels, s));
   });
 }
 
@@ -967,6 +1021,8 @@ gp_status gp_tensor_shape(gp_engine* e, const char* name, int64_t shape[4]) {
 gp_status gp_read_tensor(gp_engine* e, const char* name, float* host_out, size_t cap) {
   return guarded(e, [&]() {
     Plan* p = current_plan(e, "gp_read_tensor");
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    ArenaUse use(p, nullptr);
     GP_CUDA(cudaDeviceSynchronize());
     if (std::string(name) == "out") {
       const size_t n = (size_t)p->B * 3 * p->outH * p->outW;
@@ -1007,6 +1063,8 @@ gp_status gp_write_tensor(gp_engine* e, const char* name, const float* host_in, 
           q[0] = host_f2h(v, e->ws.bf16);
           if (t.planes == 2) q[t.C] = host_f2h(v - host_h2f(q[0], e->ws.bf16), e->ws.bf16);
         }
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    ArenaUse use(p, nullptr);   // the copy may still be in flight when it returns: later users wait for it
     GP_CUDA(cudaDeviceSynchronize());
     GP_CUDA(cudaMemcpy(p->arena + t.off, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
   });
@@ -1029,6 +1087,7 @@ gp_status gp_profile_ops(gp_engine* e, int out_channels, void* stream) {
     Plan* p = current_plan(e, "gp_profile_ops");
     if (e->cfg.readout == GP_READOUT_DPT) out_channels = 1;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    ArenaUse use(p, s);
     cudaEvent_t a, b;
     GP_CUDA(cudaEventCreate(&a));
     GP_CUDA(cudaEventCreate(&b));

@@ -275,6 +275,18 @@ class WeightStore {
   std::map<int, std::vector<std::vector<float>>> temb_cache;   // timestep -> folded bias per layer
 };
 
+// arena.cu: the per-device activation arena shared by the plans of engines with gp_set_shared_arena on.  join / leave
+// count the engines that share it (the last leave unmaps everything and frees the reservation); add maps enough for a
+// plan of `bytes` and returns the pool's fixed base, or null when the device cannot back it; remove gives a plan's share
+// back, synchronising the device before it unmaps.  wait / record order a call's stream after every earlier user of the
+// pool and every later user after the call.
+void shared_arena_join(int device);
+void shared_arena_leave(int device);
+uint8_t* shared_arena_add(int device, size_t bytes);
+void shared_arena_remove(int device, size_t bytes);
+void shared_arena_wait(int device, cudaStream_t s);
+void shared_arena_record(int device, cudaStream_t s);
+
 // builder.cu: (BN, MT) of a stride-1 implicit-GEMM layer (default policy + the waves / L2-traffic model)
 // N tile width for a GEMM with `cout` output columns (`force` != 0: that width); one of 16, 32, 64, 128.
 int choose_bn(int cout, int force);

@@ -59,6 +59,9 @@ def lib():
     L.gp_ensemble_reduce.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
     L.gp_plan_count.argtypes = [c_void_p]
     L.gp_set_memory_efficient_attention.argtypes = [c_void_p, c_int]
+    L.gp_set_shared_arena.argtypes = [c_void_p, c_int]
+    L.gp_shared_arena_info.argtypes = [c_int, POINTER(c_int64), POINTER(c_int64), POINTER(c_int64)]
+    L.gp_shared_arena_fill.argtypes = [c_int, c_int, c_void_p]
     L.gp_tile_shape.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]
     L.gp_tensor_shape.argtypes = [c_void_p, c_char_p, POINTER(c_int64)]
     L.gp_read_tensor.argtypes = [c_void_p, c_char_p, c_void_p, c_size_t]
@@ -124,7 +127,7 @@ class Engine:
     """One engine per (process, GPU).  Mirrors the C-ABI one to one."""
 
     def __init__(self, dtype=torch.float16, readout="vae", timestep=1, device=0, cuda_graph="auto",
-                 precision="default", arch="genpercept", memory_efficient_attention=False):
+                 precision="default", arch="genpercept", memory_efficient_attention=False, shared_arena=False):
         if not torch.cuda.is_available():
             raise RuntimeError("genpercept_b200 needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.L = lib()
@@ -145,6 +148,9 @@ class Engine:
         self.memory_efficient_attention = False
         if memory_efficient_attention:
             self.set_memory_efficient_attention(True)
+        self.shared_arena = False
+        if shared_arena:
+            self.set_shared_arena(True)
 
     def set_memory_efficient_attention(self, flag):
         """High-precision mode: run every attention fused, storing no T x T score matrix (gp_set_memory_efficient_attention).
@@ -154,6 +160,16 @@ class Engine:
             self.plan_shape = None
             self.out_hw = None
         self.memory_efficient_attention = bool(flag)
+
+    def set_shared_arena(self, flag):
+        """Take the activation arena of every plan from the device's one shared pool (gp_set_shared_arena), so engines
+        and cached plans that opt in need the largest arena among them, not the sum.  A shared plan's kept tensors
+        (``read_tensor``) are meaningful only straight after its own call.  A change drops the cached plans."""
+        self._ck(self.L.gp_set_shared_arena(self.h, 1 if flag else 0), "gp_set_shared_arena")
+        if bool(flag) != self.shared_arena:
+            self.plan_shape = None
+            self.out_hw = None
+        self.shared_arena = bool(flag)
 
     def close(self):
         if getattr(self, "h", None):
@@ -333,6 +349,20 @@ class Engine:
             res.append({"name": buf.value.decode(), "usec": us.value, "flops": fl.value, "bytes": by.value,
                         "kind": kd.value, "flops_exec": fx.value})
         return res
+
+
+def shared_arena_info(device=0):
+    """The device's shared activation pool: {"mapped_bytes", "reserved_bytes", "live_plans"} (all 0 when no engine on
+    `device` shares it)."""
+    m, r, n = c_int64(), c_int64(), c_int64()
+    _check_free(lib().gp_shared_arena_info(int(device), byref(m), byref(r), byref(n)), "gp_shared_arena_info")
+    return {"mapped_bytes": m.value, "reserved_bytes": r.value, "live_plans": n.value}
+
+
+def shared_arena_fill(byte, device=0):
+    """Tests: write `byte` over the shared pool's mapped range, on the current stream and ordered after every earlier
+    user of the pool (gp_shared_arena_fill)."""
+    _check_free(lib().gp_shared_arena_fill(int(device), int(byte), _stream_ptr(device)), "gp_shared_arena_fill")
 
 
 # ---------------------------------------------------------------- per-kernel entry points (tests)

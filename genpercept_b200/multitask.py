@@ -28,9 +28,13 @@ class MultiTaskPipeline:
 
     The pipelines must run the one-step arch on one device with one dtype and precision mode, and hold equal VAE encoder
     weights (vae.encoder.*, vae.quant_conv.*, compared by value); their decoders, DPT heads, UNets, timesteps and text
-    embeddings are their own.  Otherwise construction raises ValueError naming the task and what differs."""
+    embeddings are their own.  Otherwise construction raises ValueError naming the task and what differs.
 
-    def __init__(self, pipelines: Dict[str, GenPerceptPipeline], modes: Dict[str, str]):
+    ``share_arena=True`` turns on the shared activation arena (``GenPerceptPipeline.enable_shared_arena``) of every task's
+    engine, so the tasks need one inference's worth of activation memory instead of one per task; the maps are unchanged.
+    """
+
+    def __init__(self, pipelines: Dict[str, GenPerceptPipeline], modes: Dict[str, str], share_arena: bool = False):
         if not pipelines:
             raise ValueError("MultiTaskPipeline needs at least one task")
         if set(modes) != set(pipelines):
@@ -53,6 +57,9 @@ class MultiTaskPipeline:
                                      "tasks that share the VAE encoder")
         self.pipelines = dict(pipelines)
         self.modes = dict(modes)
+        if share_arena:
+            for p in self.pipelines.values():
+                p.enable_shared_arena()
 
     @torch.no_grad()
     def __call__(self, input_image, processing_res: Optional[int] = None, match_input_res: bool = True,

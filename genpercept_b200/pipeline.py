@@ -184,6 +184,16 @@ class GenPerceptPipeline:
         """Back to the default: the high-precision mode stores the score matrices (the plans ``bench.py`` measures)."""
         self._engine.set_memory_efficient_attention(False)
 
+    def enable_shared_arena(self):
+        """Take this pipeline's activation memory from the device's one shared pool, so several pipelines (or several
+        native-resolution shapes) in one process need the largest arena among them, not the sum, as the reference's
+        pipelines share PyTorch's caching allocator.  Outputs are unchanged.  Valid before or after the first inference."""
+        self._engine.set_shared_arena(True)
+
+    def disable_shared_arena(self):
+        """Back to the default: every plan owns its activation arena."""
+        self._engine.set_shared_arena(False)
+
     def set_progress_bar_config(self, **k):
         return None
 

@@ -84,6 +84,31 @@ int gp_plan_count(gp_engine* e);
  * softmax's 16384 keys fails at gp_plan with GP_ERR_INVALID.  The 16-bit modes always bound the score matrix and ignore
  * the switch.  Valid before or after gp_finalize; a change of value drops the cached plans. */
 gp_status gp_set_memory_efficient_attention(gp_engine* e, int enable);
+/* One activation arena per device for the engines that opt in, as PyTorch's caching allocator serves every pipeline of a
+ * process in the reference.  enable != 0: this engine's plans take their arena from the device's shared pool instead of
+ * a cudaMalloc of their own, so N engines (or N cached plans) need the largest arena among them, not the sum.  The pool
+ * reserves a virtual range the size of the device's memory once and maps physical memory behind a fixed base: it grows
+ * when a larger plan is made, shrinks (after a device synchronisation) when the largest plan goes, and unmaps everything
+ * when the last engine using it leaves.  A plan that does not fit fails at gp_plan with GP_ERR_INVALID, as without the
+ * pool, and the engine stays usable.  Every call that touches a shared plan's arena waits on the pool's one event on its
+ * stream first and records it after its last operation, so engines on different streams take turns without a host
+ * synchronisation.  Off by default (every path, op list, arena size and result is then as without the pool).  Valid
+ * before or after gp_finalize; a change of value synchronises and drops the cached plans.
+ * Semantics of a shared plan:
+ *   - its kept tensors ("rgb_latent", "z", "feat0".., "out" of gp_read_tensor) hold meaningful data only until another
+ *     plan in the pool runs or the pool shrinks, so gp_run_stage chains and gp_read_tensor are meaningful only straight
+ *     after the plan's own call;
+ *   - results always leave through the caller's buffer, as without the pool;
+ *   - one host thread per pool: concurrent host threads on the engines of one device are not supported. */
+gp_status gp_set_shared_arena(gp_engine* e, int enable);
+/* The device's shared pool: bytes mapped now (the largest live shared plan's arena rounded up to the allocation
+ * granularity), bytes of virtual address space reserved, and the number of live plans in it; all 0 when no engine on
+ * `device` shares it. */
+gp_status gp_shared_arena_info(int device, int64_t* mapped_bytes, int64_t* reserved_bytes, int64_t* live_plans);
+/* Tests: writes `byte` over the whole mapped range on `stream`, ordered after every earlier user of the pool and before
+ * every later one.  No op reads arena bytes it did not write in the same call, so results do not change.  GP_ERR_STATE
+ * when no engine on `device` shares the pool. */
+gp_status gp_shared_arena_fill(int device, int byte, void* stream);
 /* Host-only introspection (no device needed): the N tile (BN) and the number of 128-pixel M tiles per CTA (MT) the planner
  * gives a stride-1 ks x ks convolution / linear layer cin -> cout over `images` maps of h x w output pixels on a GPU with
  * num_sms SMs (tokens_mode != 0: one row of images * h * w tokens).  Nothing in the reference corresponds to it (PyTorch /
