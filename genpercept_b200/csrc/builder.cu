@@ -185,6 +185,59 @@ static void finalize_or_throw(IgemmParams* p, const std::string& name) {
   if (err) throw GpError(GP_ERR_INVALID, name + ": " + err);
 }
 
+// A operand view `slot` of box (64, p.TW, p.TH); in the high-precision mode also its lo plane, `lo` elements further
+// with the same strides, as view slot + 4
+void Builder::tmap_a(IgemmParams& p, int slot, const void* base, long long lo, int C, int W, int H, int N, long long sW,
+                     long long sH, long long sN, const std::string& what) const {
+  check_cuda(make_tmap_a(&p.tmA[slot], base, C, W, H, N, sW, sH, sN, p.TW, p.TH, bf16_), what);
+  if (split_)
+    check_cuda(make_tmap_a(&p.tmA[slot + 4], reinterpret_cast<const uint16_t*>(base) + lo, C, W, H, N, sW, sH, sN, p.TW, p.TH,
+                           bf16_), what + " lo");
+}
+// An activation B operand of box (64, p.BN, 1) in tmB; in the high-precision mode its lo plane, `lo` elements further, in
+// tmB2.  (Packed weights carry their lo plane along K: one tmB.)
+void Builder::tmap_b(IgemmParams& p, const void* base, long long lo, long long K, long long rows, long long Z, long long sRow,
+                     long long sZ, const std::string& what) const {
+  check_cuda(make_tmap_b(&p.tmB, base, K, rows, Z, sRow, sZ, p.BN, bf16_), what);
+  if (split_)
+    check_cuda(make_tmap_b(&p.tmB2, reinterpret_cast<const uint16_t*>(base) + lo, K, rows, Z, sRow, sZ, p.BN, bf16_), what + " lo");
+}
+// The A views past the first `used` repeat view 0 (and their lo planes view 4)
+static void fill_a_slots(IgemmParams& p, int used) {
+  for (int i = used; i < 4; ++i) {
+    p.tmA[i] = p.tmA[0];
+    p.tmA[i + 4] = p.tmA[4];
+  }
+}
+// The high-precision mode's three GEMM passes: hi*hi + lo*hi + hi*lo (A planes at tmA[0..3] / tmA[4..7]).  B's lo plane
+// follows its hi plane along K at `b_lo_k` (packed weights) or, with b_lo_k = 0, is tmB2.  `out_lo`: IgemmParams::out_lo.
+static void set_passes(IgemmParams& p, int b_lo_k, long long out_lo) {
+  p.npass = 3;
+  p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
+  p.pass_bk[0] = 0; p.pass_bk[1] = 0; p.pass_bk[2] = b_lo_k;
+  p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = b_lo_k ? 0 : 1;
+  p.out_lo = out_lo;
+}
+// A batched GEMM over one row of M tokens per batch index (the attention GEMMs and to_vT): 128 x 1 M tiles, one K segment
+// of `kchunks` 64-channel chunks, the N tile for `cout` columns.  The caller sets the batch coordinates, output and operands.
+static void token_gemm(IgemmParams& p, bool bf16, int M, int cout, int kchunks) {
+  std::memset(&p, 0, sizeof(p));
+  p.flags = bf16 ? IG_BF16 : 0;
+  p.gridW = M; p.gridH = 1; p.TW = 128; p.TH = 1; p.tw_shift = 7;
+  p.nseg[0] = 1;
+  p.seg[0][0] = IgemmSeg{0, 0, 0, (uint16_t)kchunks};
+  p.outW = M; p.outH = 1;
+  p.out_row_stride = 0;
+  p.out_sy = p.out_sx = 1;
+  p.Cout = cout;
+  p.BN = choose_bn(cout, 0);
+}
+void Builder::push_igemm(const std::string& name, IgemmParams& p, double flops, double bytes) {
+  finalize_or_throw(&p, name);
+  push(name, 1, flops, bytes, [p](cudaStream_t s) { return igemm_launch(p, s); });
+  ops.back().kind = 1;
+}
+
 // The patch-resident kernel with the GroupNorm transform in its operand path (igemm_patch.cu) takes a convolution when:
 // 3x3 stride 1, ONE normalised source (channels % 64 == 0), at most one raw shortcut source, W % 128 == 0, and either the
 // staged epilogue (Cout % 64 == 0) or an fp32 map as output.  Opt-in (GP_GN_FUSE=1) until it has been timed against the
@@ -238,14 +291,15 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   if (!a.out_f32) GP_REQUIRE(a.out.N == N && a.out.H == Ho && a.out.W == Wo, name + ": output shape mismatch");
   // GroupNorm partial sums from the epilogue: same decision (and arena allocation) in both passes
   const bool tokens_mode = (a.ks == 1 && a.mode == 0 && a.sc.empty() && a.srcs.size() == 1 && !a.out_f32);
-  const long long work_px = tokens_mode ? (long long)N * H * W
-                                        : (long long)(a.mode == 3 ? W : Wo) * (a.mode == 3 ? H : Ho) * N * (a.mode == 3 ? 4 : 1);
+  const long long ntok = (long long)N * H * W;
+  // extent of the tile grid: the output, or in mode 3 the input grid of each of the four parity classes
+  const int gw = a.mode == 3 ? W : Wo, gh = a.mode == 3 ? H : Ho;
+  const long long work_px = tokens_mode ? ntok : (long long)gw * gh * N * (a.mode == 3 ? 4 : 1);
   int bn_pre = choose_bn(Cout, a.force_bn);
   int mt_pre = (bn_pre <= 64 && work_px >= 256LL * num_sms) ? 2 : 1;
   if (!a.force_bn && !(a.flags & IG_GEGLU) && !gn_fused) {
     const double k_elems = flops / (2.0 * N * Ho * Wo * (double)Cout) * (a.mode == 3 ? 4.0 / 9.0 : 1.0);
-    tile_shape_for(Cout, k_elems, tokens_mode, N * (a.mode == 3 ? 4 : 1), (a.mode == 3) ? W : Wo, (a.mode == 3) ? H : Ho, num_sms,
-                   &bn_pre, &mt_pre);
+    tile_shape_for(Cout, k_elems, tokens_mode, N * (a.mode == 3 ? 4 : 1), gw, gh, num_sms, &bn_pre, &mt_pre);
   }
   // the staged (TMA store) epilogue wherever the output allows it; GEGLU and fp32 maps take the direct epilogue
   const bool staged = !a.out_f32 && !(a.flags & IG_GEGLU) && Cout == a.out.C && (Cout % 64) == 0 && (bn_pre % 64) == 0;
@@ -280,9 +334,8 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   p.BN = bn_pre;
   p.Z1 = 1; p.Z0 = 1;
   p.out_sy = p.out_sx = 1;
-  const bool tokens = tokens_mode;
-  if (tokens) {
-    const long long ntok = (long long)N * H * W;
+  int nmap = 0;   // A views in use
+  if (tokens_mode) {
     GP_REQUIRE(ntok < (1LL << 31), name + ": too many tokens");
     p.gridW = (int)ntok; p.gridH = 1;
     p.MT = mt_pre;
@@ -291,14 +344,7 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
     p.seg[0][0] = IgemmSeg{0, 0, 0, (uint16_t)ceil_div(s0.C, 64)};
     p.outW = (int)ntok; p.outH = 1;
     p.out_pix_stride = out_c; p.out_row_stride = 0;
-    check_cuda(make_tmap_a(&p.tmA[0], ptr(s0), s0.C, (int)ntok, 1, 1, s0.ps(), ntok * s0.ps(), ntok * s0.ps(), p.TW, 1, bf16_),
-               name + ": tmap A");
-    for (int i = 1; i < 4; ++i) p.tmA[i] = p.tmA[0];
-    if (split_) {
-      check_cuda(make_tmap_a(&p.tmA[4], reinterpret_cast<const uint16_t*>(ptr(s0)) + s0.C, s0.C, (int)ntok, 1, 1, s0.ps(),
-                             ntok * s0.ps(), ntok * s0.ps(), p.TW, 1, bf16_), name + ": tmap A lo");
-      for (int i = 5; i < 8; ++i) p.tmA[i] = p.tmA[4];
-    }
+    tmap_a(p, nmap++, ptr(s0), s0.C, s0.C, (int)ntok, 1, 1, s0.ps(), ntok * s0.ps(), ntok * s0.ps(), name + ": tmap A");
   } else {
     p.Z1 = N;
     p.a_n_z1 = 1;
@@ -306,22 +352,16 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
     p.out_pix_stride = out_c;
     p.out_row_stride = (long long)Wo * out_c;
     p.out_z1 = (long long)Ho * Wo * out_c;
-    p.gridW = (a.mode == 3) ? W : Wo;
-    p.gridH = (a.mode == 3) ? H : Ho;
+    p.gridW = gw;
+    p.gridH = gh;
     // two accumulator tiles per CTA when the N tile is narrow and there is enough work to fill the GPU
     p.MT = mt_pre;
     if (patch_eligible) { p.TW = 128; p.TH = p.MT; p.tw_shift = 7; }
     else choose_tile(p.gridW, p.gridH, 128 * p.MT, &p.TW, &p.TH, &p.tw_shift);
-    int nmap = 0;
     if (a.mode == 0 || a.mode == 3) {
       GP_REQUIRE(a.srcs.size() + a.sc.size() <= 4, name + ": too many sources");
       auto add_src = [&](const T4& s) {
-        check_cuda(make_tmap_a(&p.tmA[nmap], ptr(s), s.C, W, H, N, s.ps(), (long long)W * s.ps(),
-                               (long long)H * W * s.ps(), p.TW, p.TH, bf16_), name + ": tmap A");
-        if (split_)
-          check_cuda(make_tmap_a(&p.tmA[nmap + 4], reinterpret_cast<const uint16_t*>(ptr(s)) + s.C, s.C, W, H, N, s.ps(),
-                                 (long long)W * s.ps(), (long long)H * W * s.ps(), p.TW, p.TH, bf16_), name + ": tmap A lo");
-        ++nmap;
+        tmap_a(p, nmap++, ptr(s), s.C, s.C, W, H, N, s.ps(), (long long)W * s.ps(), (long long)H * W * s.ps(), name + ": tmap A");
       };
       for (auto& s : a.srcs) {
         GP_REQUIRE(s.N == N && s.H == H && s.W == W, name + ": source shape mismatch");
@@ -336,15 +376,11 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
       for (int hp = 0; hp < 2; ++hp)
         for (int wp = 0; wp < 2; ++wp) {
           const uint8_t* b = reinterpret_cast<const uint8_t*>(ptr(s0)) + ((long long)hp * W + wp) * s0.ps() * 2;
-          check_cuda(make_tmap_a(&p.tmA[hp * 2 + wp], b, s0.C, (W - wp + 1) / 2, (H - hp + 1) / 2, N, 2LL * s0.ps(),
-                                 2LL * W * s0.ps(), (long long)H * W * s0.ps(), p.TW, p.TH, bf16_), name + ": tmap A");
-          if (split_)
-            check_cuda(make_tmap_a(&p.tmA[4 + hp * 2 + wp], b + s0.C * 2, s0.C, (W - wp + 1) / 2, (H - hp + 1) / 2, N, 2LL * s0.ps(),
-                                   2LL * W * s0.ps(), (long long)H * W * s0.ps(), p.TW, p.TH, bf16_), name + ": tmap A lo");
+          tmap_a(p, hp * 2 + wp, b, s0.C, s0.C, (W - wp + 1) / 2, (H - hp + 1) / 2, N, 2LL * s0.ps(), 2LL * W * s0.ps(),
+                 (long long)H * W * s0.ps(), name + ": tmap A");
         }
       nmap = 4;
     }
-    for (int i = nmap; i < 4; ++i) { p.tmA[i] = p.tmA[0]; if (split_) p.tmA[i + 4] = p.tmA[4]; }
     if (a.mode == 0) {
       int ns = 0;
       const int half = a.ks / 2;
@@ -383,59 +419,38 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
       }
     }
   }
+  fill_a_slots(p, nmap);
   check_cuda(make_tmap_b(&p.tmB, a.w->w, (long long)a.w->ktot * PL, a.w->rows, a.w->nz, (long long)a.w->ktot * PL,
                          (long long)a.w->rows * a.w->ktot * PL, p.BN, bf16_), name + ": tmap B");
-  if (split_) {   // three passes: hi*hi, lo*hi, hi*lo (the weights' lo plane follows the hi plane along K)
-    p.npass = 3;
-    p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
-    p.pass_bk[0] = 0; p.pass_bk[1] = 0; p.pass_bk[2] = a.w->ktot;
-    if (!a.out_f32) p.out_lo = out_cl;
-  }
+  if (split_) set_passes(p, a.w->ktot, out_cl);   // the weights' lo plane follows the hi plane along K
   if (staged) {   // output tensor maps for the TMA-store epilogue (one per parity class)
     p.tma_store = 1;
     const int bw = p.TW < 32 ? p.TW : 32, bh = 32 / bw;
-    for (int pl = 0; pl < PL; ++pl) {          // plane 0: tmOut, plane 1 (high-precision lo): tmOutLo
-      CUtensorMap* tmo = pl == 0 ? p.tmOut : p.tmOutLo;
-      const uint8_t* obase = reinterpret_cast<const uint8_t*>(ptr(a.out)) + (size_t)pl * out_cl * 2;
-      if (tokens) {
-        const long long ntok = (long long)N * H * W;
-        check_cuda(make_tmap_a(&tmo[0], obase, out_cl, (int)ntok, 1, 1, out_c, ntok * out_c, ntok * out_c, bw, bh, bf16_),
-                   name + ": tmap out");
-        for (int i = 1; i < 4; ++i) tmo[i] = tmo[0];
-      } else if (a.mode == 3) {
+    // maps of out_cl channels at the output's pixel stride over `base`, in the output's geometry
+    auto epilogue_maps = [&](CUtensorMap* m, const uint8_t* base, const std::string& what) {
+      if (a.mode == 3) {
         for (int c = 0; c < 4; ++c) {
           const int py = c >> 1, px = c & 1;
-          const uint8_t* ob = obase + ((long long)py * Wo + px) * out_c * 2;
-          check_cuda(make_tmap_a(&tmo[c], ob, out_cl, W, H, N, 2LL * out_c, 2LL * Wo * out_c, (long long)Ho * Wo * out_c, bw, bh,
-                                 bf16_), name + ": tmap out");
+          const uint8_t* ob = base + ((long long)py * Wo + px) * out_c * 2;
+          check_cuda(make_tmap_a(&m[c], ob, out_cl, W, H, N, 2LL * out_c, 2LL * Wo * out_c, (long long)Ho * Wo * out_c, bw, bh,
+                                 bf16_), what);
         }
-      } else {
-        check_cuda(make_tmap_a(&tmo[0], obase, out_cl, Wo, Ho, N, out_c, (long long)Wo * out_c, (long long)Ho * Wo * out_c,
-                               bw, bh, bf16_), name + ": tmap out");
-        for (int i = 1; i < 4; ++i) tmo[i] = tmo[0];
+        return;
       }
-    }
-    // the residual has the output's shape and addressing: same maps over its base
+      if (tokens_mode)
+        check_cuda(make_tmap_a(&m[0], base, out_cl, (int)ntok, 1, 1, out_c, ntok * out_c, ntok * out_c, bw, bh, bf16_), what);
+      else
+        check_cuda(make_tmap_a(&m[0], base, out_cl, Wo, Ho, N, out_c, (long long)Wo * out_c, (long long)Ho * Wo * out_c,
+                               bw, bh, bf16_), what);
+      for (int i = 1; i < 4; ++i) m[i] = m[0];
+    };
+    for (int pl = 0; pl < PL; ++pl)           // plane 0: tmOut, plane 1 (high-precision lo): tmOutLo
+      epilogue_maps(pl == 0 ? p.tmOut : p.tmOutLo, reinterpret_cast<const uint8_t*>(ptr(a.out)) + (size_t)pl * out_cl * 2,
+                    name + ": tmap out");
+    // the residual has the output's shape and addressing: same maps over its base (one plane: out_c == out_cl)
     if (a.res1 && !a.res2 && !split_) {
       p.res_tma = 1;
-      const void* rb = ptr(*a.res1);
-      if (tokens) {
-        const long long ntok = (long long)N * H * W;
-        check_cuda(make_tmap_a(&p.tmRes[0], rb, out_c, (int)ntok, 1, 1, out_c, ntok * out_c, ntok * out_c, bw, bh, bf16_),
-                   name + ": tmap res");
-        for (int i = 1; i < 4; ++i) p.tmRes[i] = p.tmRes[0];
-      } else if (a.mode == 3) {
-        for (int c = 0; c < 4; ++c) {
-          const int py = c >> 1, px = c & 1;
-          const uint8_t* ob = reinterpret_cast<const uint8_t*>(rb) + ((long long)py * Wo + px) * out_c * 2;
-          check_cuda(make_tmap_a(&p.tmRes[c], ob, out_c, W, H, N, 2LL * out_c, 2LL * Wo * out_c, (long long)Ho * Wo * out_c, bw, bh,
-                                 bf16_), name + ": tmap res");
-        }
-      } else {
-        check_cuda(make_tmap_a(&p.tmRes[0], rb, out_c, Wo, Ho, N, out_c, (long long)Wo * out_c, (long long)Ho * Wo * out_c,
-                               bw, bh, bf16_), name + ": tmap res");
-        for (int i = 1; i < 4; ++i) p.tmRes[i] = p.tmRes[0];
-      }
+      epilogue_maps(p.tmRes, reinterpret_cast<const uint8_t*>(ptr(*a.res1)), name + ": tmap res");
     }
   }
   // patch-resident main loop for the wide-image, narrow-N 3x3 layers
@@ -461,7 +476,7 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   if (emit_stats) {
     p.stats = reinterpret_cast<float*>(raw_ptr(stats_off));
     p.stats_slots = num_sms;
-    p.stats_hw = tokens ? H * W : 0;
+    p.stats_hw = tokens_mode ? H * W : 0;
   }
   finalize_or_throw(&p, name);
   GP_REQUIRE(p.MT == mt_pre && p.BN == bn_pre, name + ": tile pre-selection disagrees with the plan");
@@ -469,7 +484,7 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   for (int c = 0; c < ncls; ++c)
     GP_REQUIRE(p.nkb[c] * 64 == a.w->ktot, name + ": packed K (" + std::to_string(a.w->ktot) + ") != planned K (" +
                                               std::to_string(p.nkb[c] * 64) + ")");
-  GP_REQUIRE(a.w->rows >= Cout || a.w->rows == Cout, name + ": packed rows < Cout");
+  GP_REQUIRE(a.w->rows >= Cout, name + ": packed rows < Cout");
   if (emit_stats) {
     float* sp = p.stats;
     push(name, 2, flops, bytes, [p, sp, stats_bytes](cudaStream_t s) {
@@ -491,28 +506,6 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   if (a.mode == 3) ops.back().flops_exec = flops * 4.0 / 9.0;      // four 2x2 parity convs instead of a 3x3 on the 2x grid
 }
 
-// The high-precision mode's three GEMM passes: hi*hi + lo*hi + hi*lo (A planes at tmA[0] / tmA[4], B at tmB / tmB2)
-static void set_passes(IgemmParams& p) {
-  p.npass = 3;
-  p.pass_amap[0] = 0; p.pass_amap[1] = 4; p.pass_amap[2] = 0;
-  p.pass_bmap[0] = 0; p.pass_bmap[1] = 0; p.pass_bmap[2] = 1;
-}
-
-// The lo-plane tensor maps of a fused attention kernel in the high-precision mode (FattnParams / Fattn512Params)
-template <class P>
-static void set_split_maps(P& p, const void* q, const void* k, const void* vT, int C, int T, int B, long long cs,
-                           long long qk_lo, int Tp, int q_box, int out_lo, const std::string& name) {
-  const uint16_t* ql = reinterpret_cast<const uint16_t*>(q) + qk_lo;
-  const uint16_t* kl = reinterpret_cast<const uint16_t*>(k) + qk_lo;
-  const uint16_t* vl = reinterpret_cast<const uint16_t*>(vT) + Tp;
-  const long long TpP = 2LL * Tp;
-  check_cuda(make_tmap_b(&p.tmQl, ql, C, T, B, cs, (long long)T * cs, q_box, false), name + ": tmap Q lo");
-  check_cuda(make_tmap_b(&p.tmKl, kl, C, T, B, cs, (long long)T * cs, q_box, false), name + ": tmap K lo");
-  check_cuda(make_tmap_b(&p.tmVl, vl, T, C, B, TpP, (long long)C * TpP, 64, false), name + ": tmap Vt lo");
-  p.split = 1;
-  p.out_lo = out_lo;
-}
-
 void Builder::attention_qkv(const std::string& name, const void* q, const void* k, long long cs, const void* vT, int B,
                             int T, int heads, int d, const float* pv_bias, const T4& out, long long qk_lo) {
   // High-precision mode: q / k carry their lo planes `qk_lo` elements further (same pixel stride cs), V^T rows are
@@ -524,20 +517,34 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
   // The high-precision mode takes the fused kernels only when memory-efficient attention is switched on; by default
   // its plans store S.
   const bool split_fused = split_ && mem_efficient_attn;
-  if (d == 64 && (!split_ || split_fused)) {   // fused wgmma flash-attention kernel (S and P stay on chip)
-    if (measuring_) return;
-    FattnParams p;
+  // the fused kernels' params (FattnParams / Fattn512Params) but for `heads` / `bias`: Q and K boxes of q_box tokens, and
+  // in the high-precision mode the lo planes' maps
+  auto fattn_setup = [&](auto& p, int q_box) {
     std::memset(&p, 0, sizeof(p));
     p.out = ptr(out);
     p.out_b_stride = (long long)T * out.ps();
     p.out_row_stride = (int)out.ps();
-    p.T = T; p.heads = heads; p.B = B; p.q_tiles = ceil_div(T, 128);
+    p.T = T; p.B = B; p.q_tiles = ceil_div(T, q_box);
     p.scale_log2e = 1.4426950408889634f;
     p.bf16 = bf16_ ? 1 : 0;
-    check_cuda(make_tmap_b(&p.tmQ, q, C, T, B, cs, (long long)T * cs, 128, bf16_), name + ": tmap Q");
-    check_cuda(make_tmap_b(&p.tmK, k, C, T, B, cs, (long long)T * cs, 128, bf16_), name + ": tmap K");
+    check_cuda(make_tmap_b(&p.tmQ, q, C, T, B, cs, (long long)T * cs, q_box, bf16_), name + ": tmap Q");
+    check_cuda(make_tmap_b(&p.tmK, k, C, T, B, cs, (long long)T * cs, q_box, bf16_), name + ": tmap K");
     check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, TpP, (long long)C * TpP, 64, bf16_), name + ": tmap Vt");
-    if (split_) set_split_maps(p, q, k, vT, C, T, B, cs, qk_lo, Tp, 128, out.C, name);
+    if (!split_) return;
+    const uint16_t* ql = reinterpret_cast<const uint16_t*>(q) + qk_lo;
+    const uint16_t* kl = reinterpret_cast<const uint16_t*>(k) + qk_lo;
+    const uint16_t* vl = reinterpret_cast<const uint16_t*>(vT) + Tp;
+    check_cuda(make_tmap_b(&p.tmQl, ql, C, T, B, cs, (long long)T * cs, q_box, false), name + ": tmap Q lo");
+    check_cuda(make_tmap_b(&p.tmKl, kl, C, T, B, cs, (long long)T * cs, q_box, false), name + ": tmap K lo");
+    check_cuda(make_tmap_b(&p.tmVl, vl, T, C, B, TpP, (long long)C * TpP, 64, false), name + ": tmap Vt lo");
+    p.split = 1;
+    p.out_lo = out.C;
+  };
+  if (d == 64 && (!split_ || split_fused)) {   // fused wgmma flash-attention kernel (S and P stay on chip)
+    if (measuring_) return;
+    FattnParams p;
+    fattn_setup(p, 128);
+    p.heads = heads;
     push(name + ".fattn", 1, 4.0 * B * heads * (double)T * T * d, 4.0 * B * T * C * 2 * PL,
          [p](cudaStream_t s) { return fattn_launch(p, s); });
     ops.back().kind = 2;
@@ -552,18 +559,8 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
   if (fused512) {   // fused d = 512 kernel: no score matrix in the arena
     if (measuring_) return;
     Fattn512Params p;
-    std::memset(&p, 0, sizeof(p));
-    p.out = ptr(out);
+    fattn_setup(p, 64);
     p.bias = pv_bias;
-    p.out_b_stride = (long long)T * out.ps();
-    p.out_row_stride = (int)out.ps();
-    p.T = T; p.B = B; p.q_tiles = ceil_div(T, 64);
-    p.scale_log2e = 1.4426950408889634f;
-    p.bf16 = bf16_ ? 1 : 0;
-    check_cuda(make_tmap_b(&p.tmQ, q, C, T, B, cs, (long long)T * cs, 64, bf16_), name + ": tmap Q");
-    check_cuda(make_tmap_b(&p.tmK, k, C, T, B, cs, (long long)T * cs, 64, bf16_), name + ": tmap K");
-    check_cuda(make_tmap_b(&p.tmV, vT, T, C, B, TpP, (long long)C * TpP, 64, bf16_), name + ": tmap Vt");
-    if (split_) set_split_maps(p, q, k, vT, C, T, B, cs, qk_lo, Tp, 64, out.C, name);
     push(name + ".fattn512", 1, 4.0 * B * (double)T * T * d, 4.0 * B * T * C * 2 * PL,
          [p](cudaStream_t s) { return fattn512_launch(p, s); });
     ops.back().kind = 2;
@@ -575,36 +572,18 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
     void* S = raw_ptr(s_off);
     {  // S = Q K^T  (softmax scale is folded into Wq)
       IgemmParams p;
-      std::memset(&p, 0, sizeof(p));
-      p.flags = bf16_ ? IG_BF16 : 0;
-      p.gridW = T; p.gridH = 1; p.TW = 128; p.TH = 1; p.tw_shift = 7;
+      token_gemm(p, bf16_, T, T, ceil_div(d, 64));
       p.Z1 = B; p.Z0 = heads;
       p.a_n_z1 = 1; p.a_k_z0 = d;
       p.b_z_z1 = 1; p.b_k_z0 = d;
-      p.nseg[0] = 1;
-      p.seg[0][0] = IgemmSeg{0, 0, 0, (uint16_t)ceil_div(d, 64)};
-      p.out = S; p.outW = T; p.outH = 1;
-      p.out_pix_stride = TpP; p.out_row_stride = 0;
+      p.out = S;
+      p.out_pix_stride = TpP;
       p.out_z1 = (long long)heads * T * TpP; p.out_z0 = (long long)T * TpP;
-      p.out_sy = p.out_sx = 1;
-      p.Cout = T;
-      p.BN = choose_bn(T, 0);
-      check_cuda(make_tmap_a(&p.tmA[0], q, C, T, 1, B, cs, (long long)T * cs, (long long)T * cs, 128, 1, bf16_), name + ": tmap Q");
-      for (int i = 1; i < 4; ++i) p.tmA[i] = p.tmA[0];
-      check_cuda(make_tmap_b(&p.tmB, k, C, T, B, cs, (long long)T * cs, p.BN, bf16_), name + ": tmap K");
-      if (split_) {
-        const uint16_t* ql = reinterpret_cast<const uint16_t*>(q) + qk_lo;
-        const uint16_t* kl = reinterpret_cast<const uint16_t*>(k) + qk_lo;
-        check_cuda(make_tmap_a(&p.tmA[4], ql, C, T, 1, B, cs, (long long)T * cs, (long long)T * cs, 128, 1, bf16_), name + ": tmap Q lo");
-        for (int i = 5; i < 8; ++i) p.tmA[i] = p.tmA[4];
-        check_cuda(make_tmap_b(&p.tmB2, kl, C, T, B, cs, (long long)T * cs, p.BN, bf16_), name + ": tmap K lo");
-        p.out_lo = Tp;
-        set_passes(p);
-      }
-      finalize_or_throw(&p, name + ".qk");
-      push(name + ".qk", 1, 2.0 * B * heads * (double)T * T * d, (double)s_bytes + 2.0 * B * T * C * 2,
-           [p](cudaStream_t s) { return igemm_launch(p, s); });
-      ops.back().kind = 1;
+      tmap_a(p, 0, q, qk_lo, C, T, 1, B, cs, (long long)T * cs, (long long)T * cs, name + ": tmap Q");
+      fill_a_slots(p, 1);
+      tmap_b(p, k, qk_lo, C, T, B, cs, (long long)T * cs, name + ": tmap K");
+      if (split_) set_passes(p, 0, Tp);
+      push_igemm(name + ".qk", p, 2.0 * B * heads * (double)T * T * d, (double)s_bytes + 2.0 * B * T * C * 2);
     }
     {
       const long long rows = (long long)B * heads * T;
@@ -614,37 +593,19 @@ void Builder::attention_qkv(const std::string& name, const void* q, const void* 
     }
     {  // O = P V
       IgemmParams p;
-      std::memset(&p, 0, sizeof(p));
-      p.flags = bf16_ ? IG_BF16 : 0;
-      p.gridW = T; p.gridH = 1; p.TW = 128; p.TH = 1; p.tw_shift = 7;
+      token_gemm(p, bf16_, T, d, ceil_div(T, 64));
       p.Z1 = B; p.Z0 = heads;
       p.a_n_z1 = heads; p.a_n_z0 = 1;
       p.b_z_z1 = 1; p.b_row_z0 = d;
-      p.nseg[0] = 1;
-      p.seg[0][0] = IgemmSeg{0, 0, 0, (uint16_t)ceil_div(T, 64)};
-      p.out = ptr(out); p.outW = T; p.outH = 1;
-      p.out_pix_stride = out.ps(); p.out_row_stride = 0;
+      p.out = ptr(out);
+      p.out_pix_stride = out.ps();
       p.out_z1 = (long long)T * out.ps(); p.out_z0 = d;
-      p.out_sy = p.out_sx = 1;
-      p.Cout = d;
       p.bias = pv_bias;
-      p.BN = choose_bn(d, 0);
-      check_cuda(make_tmap_a(&p.tmA[0], S, T, T, 1, B * heads, TpP, (long long)T * TpP, (long long)T * TpP, 128, 1, bf16_), name + ": tmap P");
-      for (int i = 1; i < 4; ++i) p.tmA[i] = p.tmA[0];
-      check_cuda(make_tmap_b(&p.tmB, vT, T, C, B, TpP, (long long)C * TpP, p.BN, bf16_), name + ": tmap Vt");
-      if (split_) {
-        check_cuda(make_tmap_a(&p.tmA[4], reinterpret_cast<const uint16_t*>(S) + Tp, T, T, 1, B * heads, TpP, (long long)T * TpP,
-                               (long long)T * TpP, 128, 1, bf16_), name + ": tmap P lo");
-        for (int i = 5; i < 8; ++i) p.tmA[i] = p.tmA[4];
-        check_cuda(make_tmap_b(&p.tmB2, reinterpret_cast<const uint16_t*>(vT) + Tp, T, C, B, TpP, (long long)C * TpP, p.BN, bf16_),
-                   name + ": tmap Vt lo");
-        p.out_lo = out.C;
-        set_passes(p);
-      }
-      finalize_or_throw(&p, name + ".pv");
-      push(name + ".pv", 1, 2.0 * B * heads * (double)T * T * d, (double)s_bytes + 2.0 * B * T * C * 2,
-           [p](cudaStream_t s) { return igemm_launch(p, s); });
-      ops.back().kind = 1;
+      tmap_a(p, 0, S, Tp, T, T, 1, B * heads, TpP, (long long)T * TpP, (long long)T * TpP, name + ": tmap P");
+      fill_a_slots(p, 1);
+      tmap_b(p, vT, Tp, T, C, B, TpP, (long long)C * TpP, name + ": tmap Vt");
+      if (split_) set_passes(p, 0, out.C);
+      push_igemm(name + ".pv", p, 2.0 * B * heads * (double)T * T * d, (double)s_bytes + 2.0 * B * T * C * 2);
     }
   }
   arena_.release(s_off);
@@ -681,85 +642,68 @@ void Builder::to_vT(const std::string& name, const T4& l, const PackedW& wv, voi
   const long long TpP = (long long)Tp * PL;
   const size_t vt_bytes = (size_t)B * C * TpP * 2;
   IgemmParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.flags = bf16_ ? IG_BF16 : 0;
-  p.gridW = C; p.gridH = 1; p.TW = 128; p.TH = 1; p.tw_shift = 7;
+  token_gemm(p, bf16_, C, T, wv.ktot / 64);
   p.Z1 = B; p.Z0 = 1;
   p.b_z_z1 = 1;
-  p.nseg[0] = 1;
-  p.seg[0][0] = IgemmSeg{0, 0, 0, (uint16_t)(wv.ktot / 64)};
-  p.out = vT; p.outW = C; p.outH = 1;
-  p.out_pix_stride = TpP; p.out_row_stride = 0;
+  p.out = vT;
+  p.out_pix_stride = TpP;
   p.out_z1 = (long long)C * TpP;
-  p.out_sy = p.out_sx = 1;
-  p.Cout = T;
-  p.BN = choose_bn(T, 0);
   const long long wrow = (long long)wv.ktot * PL;
-  check_cuda(make_tmap_a(&p.tmA[0], wv.w, wv.ktot, C, 1, 1, wrow, (long long)C * wrow, (long long)C * wrow,
-                         128, 1, bf16_), name + ": tmap Wv");
-  for (int i = 1; i < 4; ++i) p.tmA[i] = p.tmA[0];
-  check_cuda(make_tmap_b(&p.tmB, ptr(l), C, T, B, l.ps(), (long long)T * l.ps(), p.BN, bf16_), name + ": tmap l");
-  if (split_) {
-    check_cuda(make_tmap_a(&p.tmA[4], wv.w + wv.ktot, wv.ktot, C, 1, 1, wrow, (long long)C * wrow, (long long)C * wrow,
-                           128, 1, bf16_), name + ": tmap Wv lo");
-    for (int i = 5; i < 8; ++i) p.tmA[i] = p.tmA[4];
-    check_cuda(make_tmap_b(&p.tmB2, reinterpret_cast<const uint16_t*>(ptr(l)) + C, C, T, B, l.ps(), (long long)T * l.ps(), p.BN, bf16_),
-               name + ": tmap l lo");
-    set_passes(p);
-    p.out_lo = Tp;
-  }
-  finalize_or_throw(&p, name + ".to_vT");
-  push(name + ".to_vT", 1, 2.0 * B * (double)T * C * C, (double)vt_bytes + (double)l.bytes(),
-       [p](cudaStream_t s) { return igemm_launch(p, s); });
-  ops.back().kind = 1;
+  tmap_a(p, 0, wv.w, wv.ktot, wv.ktot, C, 1, 1, wrow, (long long)C * wrow, (long long)C * wrow, name + ": tmap Wv");
+  fill_a_slots(p, 1);
+  tmap_b(p, ptr(l), C, C, T, B, l.ps(), (long long)T * l.ps(), name + ": tmap l");
+  if (split_) set_passes(p, 0, Tp);
+  push_igemm(name + ".to_vT", p, 2.0 * B * (double)T * C * C, (double)vt_bytes + (double)l.bytes());
 }
 
-void Builder::gn_scale_shift(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps) {
-  int ctot = 0;
-  for (auto& s : srcs) ctot += s.C;
-  GP_REQUIRE(nw.C == ctot && ctot % groups == 0 && srcs.size() <= 2 && !srcs.empty(), name + ": GroupNorm channel mismatch");
-  const int N = srcs[0].N;
-  const long long HW = (long long)srcs[0].H * srcs[0].W;
+// GroupNorm statistics of concat(srcs) over N images of HW pixels -> scale / shift in gn_ss.  Each source's partial sums
+// are either already produced by the conv that wrote it, or computed by a gn_stats pass into a buffer of this op's own
+// (allocated and released here, so both passes make the same arena allocations).  Returns the gn_stats passes +
+// gn_finalize as one launch (empty when measuring); each gn_stats pass adds to `launches` and `bytes`.
+std::function<cudaError_t(cudaStream_t)> Builder::gn_statistics(const std::vector<T4>& srcs, const NormW& nw, int groups,
+                                                                float eps, int N, long long HW, int ctot, int* launches,
+                                                                double* bytes) {
   const int chunks = gn_chunks(N, HW);
-  std::vector<size_t> own(srcs.size(), (size_t)-1);
+  struct Pass { const void* x; float* partial; int C; };
+  std::vector<Pass> passes;
+  std::vector<size_t> own;
   std::vector<GnSrc> gs(srcs.size());
   for (size_t i = 0; i < srcs.size(); ++i) {
     auto it = stats.find(srcs[i].off);
     if (it != stats.end() && it->second.C == srcs[i].C) {
       gs[i] = GnSrc{measuring_ ? nullptr : reinterpret_cast<const float*>(raw_ptr(it->second.off)), it->second.slots, srcs[i].C};
     } else {
-      own[i] = arena_.alloc((size_t)N * chunks * srcs[i].C * 2 * sizeof(float));
-      gs[i] = GnSrc{measuring_ ? nullptr : reinterpret_cast<const float*>(raw_ptr(own[i])), chunks, srcs[i].C};
+      own.push_back(arena_.alloc((size_t)N * chunks * srcs[i].C * 2 * sizeof(float)));
+      float* partial = measuring_ ? nullptr : reinterpret_cast<float*>(raw_ptr(own.back()));
+      gs[i] = GnSrc{partial, chunks, srcs[i].C};
+      if (!measuring_) passes.push_back(Pass{ptr(srcs[i]), partial, srcs[i].C});
+      ++*launches;
+      *bytes += (double)srcs[i].bytes();
     }
   }
-  if (!measuring_) {
-    float* ss = gn_ss;
-    const bool bf = bf16_, sp = split_;
-    std::vector<const void*> xs;
-    std::vector<int> cs;
-    std::vector<bool> need;
-    int launches = 1;
-    double bytes = 0;
-    for (size_t i = 0; i < srcs.size(); ++i) {
-      xs.push_back(ptr(srcs[i]));
-      cs.push_back(srcs[i].C);
-      need.push_back(own[i] != (size_t)-1);
-      if (need[i]) { bytes += (double)srcs[i].bytes(); ++launches; }
+  for (size_t off : own) arena_.release(off);
+  if (measuring_) return nullptr;
+  float* ss = gn_ss;
+  const bool bf = bf16_, sp = split_;
+  const float* gamma = nw.gamma;
+  const float* beta = nw.beta;
+  return [=](cudaStream_t s) {
+    for (const Pass& q : passes) {
+      cudaError_t e = gn_stats(q.x, N, HW, q.C, q.partial, chunks, q.C, 0, bf, s, sp);
+      if (e != cudaSuccess) return e;
     }
-    const float* gamma = nw.gamma;
-    const float* beta = nw.beta;
-    push(name, launches, 0, bytes, [=](cudaStream_t s) {
-      cudaError_t e;
-      for (size_t i = 0; i < xs.size(); ++i) {
-        if (!need[i]) continue;
-        e = gn_stats(xs[i], N, HW, cs[i], const_cast<float*>(gs[i].partial), chunks, cs[i], 0, bf, s, sp);
-        if (e != cudaSuccess) return e;
-      }
-      return gn_finalize(gs.data(), (int)gs.size(), gamma, beta, N, ctot, groups, HW, eps, ss, s);
-    });
-  }
-  for (size_t i = 0; i < srcs.size(); ++i)
-    if (own[i] != (size_t)-1) arena_.release(own[i]);
+    return gn_finalize(gs.data(), (int)gs.size(), gamma, beta, N, ctot, groups, HW, eps, ss, s);
+  };
+}
+
+void Builder::gn_scale_shift(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps) {
+  int ctot = 0;
+  for (auto& s : srcs) ctot += s.C;
+  GP_REQUIRE(nw.C == ctot && ctot % groups == 0 && srcs.size() <= 2 && !srcs.empty(), name + ": GroupNorm channel mismatch");
+  int launches = 1;
+  double bytes = 0;
+  auto stats_fn = gn_statistics(srcs, nw, groups, eps, srcs[0].N, (long long)srcs[0].H * srcs[0].W, ctot, &launches, &bytes);
+  if (!measuring_) push(name, launches, 0, bytes, std::move(stats_fn));
 }
 
 void Builder::gn(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps,
@@ -769,58 +713,33 @@ void Builder::gn(const std::string& name, const std::vector<T4>& srcs, const Nor
   GP_REQUIRE(ctot == out.C && nw.C == ctot && ctot % groups == 0 && srcs.size() <= 2, name + ": GroupNorm channel mismatch");
   const int N = out.N;
   const long long HW = (long long)out.H * out.W;
-  const int chunks = gn_chunks(N, HW);
-  // per source: partial sums either already produced by the conv that wrote it, or computed here
-  std::vector<size_t> own(srcs.size(), (size_t)-1);
-  std::vector<GnSrc> gs(srcs.size());
-  for (size_t i = 0; i < srcs.size(); ++i) {
-    auto it = stats.find(srcs[i].off);
-    if (it != stats.end() && it->second.C == srcs[i].C) {
-      gs[i] = GnSrc{measuring_ ? nullptr : reinterpret_cast<const float*>(raw_ptr(it->second.off)), it->second.slots, srcs[i].C};
-    } else {
-      own[i] = arena_.alloc((size_t)N * chunks * srcs[i].C * 2 * sizeof(float));
-      gs[i] = GnSrc{measuring_ ? nullptr : reinterpret_cast<const float*>(raw_ptr(own[i])), chunks, srcs[i].C};
-    }
+  int launches = 1;
+  double bytes = (double)out.bytes();
+  auto stats_fn = gn_statistics(srcs, nw, groups, eps, N, HW, ctot, &launches, &bytes);
+  if (measuring_) return;
+  // then one apply pass per source
+  std::vector<const void*> xs;
+  std::vector<int> cs;
+  for (auto& s : srcs) {
+    xs.push_back(ptr(s));
+    cs.push_back(s.C);
+    bytes += (double)s.bytes();
+    ++launches;
   }
-  if (!measuring_) {
-    float* ss = gn_ss;
-    const bool bf = bf16_;
-    std::vector<const void*> xs;
-    std::vector<int> cs;
-    std::vector<bool> need;
-    int launches = 1;
-    double bytes = (double)out.bytes();
-    for (size_t i = 0; i < srcs.size(); ++i) {
-      xs.push_back(ptr(srcs[i]));
-      cs.push_back(srcs[i].C);
-      need.push_back(own[i] != (size_t)-1);
-      bytes += (need[i] ? 2.0 : 1.0) * srcs[i].bytes();
-      launches += need[i] ? 2 : 1;
-    }
-    void* y = ptr(out);
-    const float* gamma = nw.gamma;
-    const float* beta = nw.beta;
-    const bool sp = split_;
-    push(name, launches, 0, bytes, [=](cudaStream_t s) {
-      cudaError_t e;
-      for (size_t i = 0; i < xs.size(); ++i) {
-        if (!need[i]) continue;
-        e = gn_stats(xs[i], N, HW, cs[i], const_cast<float*>(gs[i].partial), chunks, cs[i], 0, bf, s, sp);
-        if (e != cudaSuccess) return e;
-      }
-      e = gn_finalize(gs.data(), (int)gs.size(), gamma, beta, N, ctot, groups, HW, eps, ss, s);
+  void* y = ptr(out);
+  float* ss = gn_ss;
+  const bool bf = bf16_, sp = split_;
+  push(name, launches, 0, bytes, [=](cudaStream_t s) {
+    cudaError_t e = stats_fn(s);
+    if (e != cudaSuccess) return e;
+    int coff = 0;
+    for (size_t i = 0; i < xs.size(); ++i) {
+      e = gn_apply(xs[i], N, HW, cs[i], ss, ctot, coff, y, ctot, silu, bf, s, sp);
       if (e != cudaSuccess) return e;
-      int coff = 0;
-      for (size_t i = 0; i < xs.size(); ++i) {
-        e = gn_apply(xs[i], N, HW, cs[i], ss, ctot, coff, y, ctot, silu, bf, s, sp);
-        if (e != cudaSuccess) return e;
-        coff += cs[i];
-      }
-      return cudaSuccess;
-    });
-  }
-  for (size_t i = 0; i < srcs.size(); ++i)
-    if (own[i] != (size_t)-1) arena_.release(own[i]);
+      coff += cs[i];
+    }
+    return cudaSuccess;
+  });
 }
 
 void Builder::ln(const std::string& name, const T4& x, const NormW& nw, float eps, const T4& out) {

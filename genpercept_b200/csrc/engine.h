@@ -188,6 +188,15 @@ class Builder {
  private:
   void push(const std::string& name, int launches, double flops, double bytes,
             std::function<cudaError_t(cudaStream_t)> fn);
+  // finalize p, push its launch, mark the op as an implicit GEMM
+  void push_igemm(const std::string& name, IgemmParams& p, double flops, double bytes);
+  // GEMM operand tensor maps, with the high-precision mode's lo plane `lo` elements after the hi plane (builder.cu)
+  void tmap_a(IgemmParams& p, int slot, const void* base, long long lo, int C, int W, int H, int N, long long sW, long long sH,
+              long long sN, const std::string& what) const;
+  void tmap_b(IgemmParams& p, const void* base, long long lo, long long K, long long rows, long long Z, long long sRow,
+              long long sZ, const std::string& what) const;
+  std::function<cudaError_t(cudaStream_t)> gn_statistics(const std::vector<T4>& srcs, const NormW& nw, int groups, float eps,
+                                                         int N, long long HW, int ctot, int* launches, double* bytes);
   bool bf16_, measuring_, split_ = false;
   uint8_t* base_;
   Arena arena_;
