@@ -278,6 +278,11 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   const int out_cl = a.out_f32 ? 0 : a.out.C;   // logical channels of the 16-bit output ...
   const int out_c = out_cl * PL;                // ... and its pixel stride in elements
   GP_REQUIRE(a.w->planes == PL, name + ": packed weights do not match the engine's precision mode");
+  if (split_) {   // a source's lo plane starts C elements into the pixel: a TMA base must be 16-byte aligned
+    for (auto& s : a.srcs) GP_REQUIRE(s.C % 8 == 0, name + ": the (hi, lo) layout needs source channels % 8 == 0");
+    for (auto& s : a.sc) GP_REQUIRE(s.C % 8 == 0, name + ": the (hi, lo) layout needs shortcut channels % 8 == 0");
+    GP_REQUIRE(!(a.flags & IG_GEGLU) || out_cl % 8 == 0, name + ": the (hi, lo) GEGLU output needs channels % 8 == 0");
+  }
   const int Cout = a.cout_valid > 0 ? a.cout_valid : a.out.C;
   int cin_total = 0;
   for (auto& s : a.srcs) cin_total += s.C;
@@ -315,7 +320,7 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   bool emit_stats = a.want_stats && staged && Cout <= 512 && !split_;
   if (emit_stats && tokens_mode && ((long long)H * W) % (128 * mt_pre) != 0) emit_stats = false;
   size_t stats_off = 0;
-  const size_t stats_bytes = (size_t)N * num_sms * Cout * 2 * sizeof(float);
+  const size_t stats_bytes = (size_t)N * num_sms * Cout * kGnRec * sizeof(float);
   if (emit_stats) {
     GP_REQUIRE(stats.find(a.out.off) == stats.end(), name + ": output already has statistics");
     stats_off = arena_.alloc(stats_bytes);
@@ -673,7 +678,7 @@ std::function<cudaError_t(cudaStream_t)> Builder::gn_statistics(const std::vecto
     if (it != stats.end() && it->second.C == srcs[i].C) {
       gs[i] = GnSrc{measuring_ ? nullptr : reinterpret_cast<const float*>(raw_ptr(it->second.off)), it->second.slots, srcs[i].C};
     } else {
-      own.push_back(arena_.alloc((size_t)N * chunks * srcs[i].C * 2 * sizeof(float)));
+      own.push_back(arena_.alloc((size_t)N * chunks * srcs[i].C * kGnRec * sizeof(float)));
       float* partial = measuring_ ? nullptr : reinterpret_cast<float*>(raw_ptr(own.back()));
       gs[i] = GnSrc{partial, chunks, srcs[i].C};
       if (!measuring_) passes.push_back(Pass{ptr(srcs[i]), partial, srcs[i].C});

@@ -99,7 +99,7 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_kernel(const __grid_con
   uint64_t* tempty_bar = tfull_bar + 1;
   uint64_t* res_bar = tempty_bar + 1;                                  // [epilogue warps] residual tile landed
   float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(res_bar + kEpiWarps) + 15) & ~uintptr_t(15));   // [bias_slots]
-  float* sacc = sbias + p.bias_slots;   // [4 epilogue warps][Cout][2], only with p.stats
+  float* sacc = sbias + p.bias_slots;   // [4 epilogue warps][Cout][2] + [4][8] counts, only with p.stats
 
   const int warp = uniform_warp_id();
   const int lane = threadIdx.x & 31;
@@ -283,7 +283,7 @@ const char* igemm_finalize(IgemmParams* p) {
   long long total = (long long)p->n_tiles_n * p->tiles_x * p->tiles_y * p->Z0 * p->Z1;
   if (total > 0x7fffffffLL) return "too many tiles";
   p->total_tiles = (int)total;
-  const int stats_bytes = p->stats ? 4 * p->Cout * 2 * (int)sizeof(float) : 0;
+  const int stats_bytes = p->stats ? (kEpiWarps * p->Cout * 2 + kEpiWarps * 8) * (int)sizeof(float) : 0;   // epilogue_staged
   if (p->tma_store && ((p->Cout % 64) || (p->BN % 64) || (p->flags & (IG_OUT_F32_NCHW | IG_GEGLU)) || p->out_z0 != 0))
     return "staged epilogue needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output, no GEGLU";
   if (p->stats && (!p->tma_store || p->Cout > 512)) return "statistics need the staged epilogue and Cout <= 512";

@@ -78,8 +78,8 @@ struct IgemmParams {
   int stages;
   int total_tiles;
   // Optional GroupNorm statistics of the (rounded) output, produced by the epilogue: per image and
-  // per CTA slot, per-channel sum / sum of squares, fp32, fixed summation order (deterministic):
-  //   stats[((image * stats_slots + blockIdx.x) * Cout + c) * 2 + {0, 1}]
+  // per CTA slot, per-channel (count, mean, M2) records (kernels.h, kGnRec), fp32, fixed merge order (deterministic):
+  //   stats[((image * stats_slots + blockIdx.x) * Cout + c) * 3 + {0, 1, 2}]
   // Pre-zeroed by the caller (CTAs that see no tile of an image do not write its slot).
   float* stats;
   int stats_slots;               // >= gridDim.x (min(total_tiles, SM count), igemm_launch)

@@ -20,6 +20,7 @@
 #include <cuda_fp16.h>
 
 #include "igemm.h"
+#include "kernels.h"
 #include "ptx.cuh"
 
 namespace gp {
@@ -218,19 +219,33 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
   const int etid = threadIdx.x;
   int cur_img = -1;
   int cur_nt = -1;
-  // sum the four warp-private accumulators in a fixed order, publish this CTA's slot, reset
+  // Statistics scratch: sacc[warp][Cout] (mean, M2) and scnt[warp][64-channel group] the count behind them (the same for
+  // every channel of a group: a warp sees the same rows for all of them).  Merge the four warps' records in a fixed
+  // order, publish this CTA's slot, reset.
+  auto scnt = [&](int i) -> float& { return sacc[kEpiWarps * 2 * p.Cout + i]; };   // derived, not kept live
   auto flush_stats = [&](int img) {
     epi_sync();
-    float* dst = p.stats + ((long long)img * p.stats_slots + blockIdx.x) * p.Cout * 2;
-    for (int i = etid; i < 2 * p.Cout; i += kEpiWarps * 32) {
-      const float tot = (sacc[i] + sacc[2 * p.Cout + i]) + (sacc[4 * p.Cout + i] + sacc[6 * p.Cout + i]);
-      dst[i] = tot;
-      sacc[i] = 0.f; sacc[2 * p.Cout + i] = 0.f; sacc[4 * p.Cout + i] = 0.f; sacc[6 * p.Cout + i] = 0.f;
+    float* dst = p.stats + ((long long)img * p.stats_slots + blockIdx.x) * p.Cout * kGnRec;
+    for (int c = etid; c < p.Cout; c += kEpiWarps * 32) {
+      float r[kEpiWarps][3];
+#pragma unroll
+      for (int w = 0; w < kEpiWarps; ++w) {
+        r[w][0] = scnt(w * 8 + (c >> 6));
+        r[w][1] = sacc[(w * p.Cout + c) * 2];
+        r[w][2] = sacc[(w * p.Cout + c) * 2 + 1];
+        sacc[(w * p.Cout + c) * 2] = 0.f; sacc[(w * p.Cout + c) * 2 + 1] = 0.f;
+      }
+      chan_merge(r[0][0], r[0][1], r[0][2], r[1][0], r[1][1], r[1][2]);
+      chan_merge(r[2][0], r[2][1], r[2][2], r[3][0], r[3][1], r[3][2]);
+      chan_merge(r[0][0], r[0][1], r[0][2], r[2][0], r[2][1], r[2][2]);
+      dst[c * kGnRec] = r[0][0]; dst[c * kGnRec + 1] = r[0][1]; dst[c * kGnRec + 2] = r[0][2];
     }
+    epi_sync();
+    if (etid < kEpiWarps * 8) scnt(etid) = 0.f;
     epi_sync();
   };
   if (do_stats) {
-    for (int i = etid; i < 8 * p.Cout; i += kEpiWarps * 32) sacc[i] = 0.f;
+    for (int i = etid; i < 8 * p.Cout + kEpiWarps * 8; i += kEpiWarps * 32) sacc[i] = 0.f;
     epi_sync();
   }
   if (p.bias_all) load_bias_tile(p, sbias, 0, etid);
@@ -299,7 +314,6 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
                          : "r"(my_row + ((i ^ sw) << 4)));
           __syncwarp();                                       // every row is in registers before the tile is overwritten
         }
-        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
         uint32_t rh[2][32];                                   // this row's accumulators of the two 32-column pieces
 #pragma unroll
         for (int sub = 0; sub < 2; ++sub) {
@@ -395,18 +409,39 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
           tma_store_commit();
         }
         if (do_stats) {
-          // lane l owns channels n0 + 2l, n0 + 2l + 1: one 32-bit word per staged row
-          const uint32_t col = stg_addr + (lane & 3) * 4;
-          const int chunk = lane >> 2;
+          // lane l owns channels n0 + 2l, n0 + 2l + 1: one 32-bit word per staged row.  The rows inside the image (bit rr
+          // of `rows`) are summed as deviations from the first of them, which keeps the piece's M2 free of cancellation;
+          // the piece's (count, mean, M2) is then merged into the warp's record.
+          const uint32_t rows = __ballot_sync(0xffffffffu, valid);
+          if (rows) {
+            const uint32_t col = stg_addr + (lane & 3) * 4;
+            const int chunk = lane >> 2;
+            auto ld = [&](int rr, float& a, float& b) {
+              uint32_t w;
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(col + rr * 128 + ((chunk ^ (rr & 7)) << 4)));
+              a = cvt16<BF16>((uint16_t)(w & 0xFFFF)); b = cvt16<BF16>((uint16_t)(w >> 16));
+            };
+            float k0, k1, s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+            ld(__ffs(rows) - 1, k0, k1);
 #pragma unroll 8
-          for (int rr = 0; rr < 32; ++rr) {
-            uint32_t w;
-            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(col + rr * 128 + ((chunk ^ (rr & 7)) << 4)));
-            const float a = cvt16<BF16>((uint16_t)(w & 0xFFFF)), b = cvt16<BF16>((uint16_t)(w >> 16));
-            s0 += a; q0 += a * a; s1 += b; q1 += b * b;
+            for (int rr = 0; rr < 32; ++rr) {
+              float a, b;
+              ld(rr, a, b);
+              const bool in = (rows >> rr) & 1u;
+              a = in ? a - k0 : 0.f; b = in ? b - k1 : 0.f;
+              s0 += a; q0 = fmaf(a, a, q0); s1 += b; q1 = fmaf(b, b, q1);
+            }
+            const float cnt = (float)__popc(rows), inv = __fdividef(1.f, cnt);
+            float& cp = scnt(wq * 8 + (n0 >> 6));
+            const float na = cp;
+            float* d = sacc + ((size_t)wq * p.Cout + n0 + 2 * lane) * 2;
+            float n_0 = na, n_1 = na;
+            chan_merge(n_0, d[0], d[1], cnt, fmaf(s0, inv, k0), fmaxf(q0 - s0 * s0 * inv, 0.f));
+            chan_merge(n_1, d[2], d[3], cnt, fmaf(s1, inv, k1), fmaxf(q1 - s1 * s1 * inv, 0.f));
+            __syncwarp();
+            if (lane == 0) cp = na + cnt;
+            __syncwarp();
           }
-          float* d = sacc + ((size_t)wq * p.Cout + n0 + 2 * lane) * 2;
-          d[0] += s0; d[1] += q0; d[2] += s1; d[3] += q1;
         }
       }
     }
@@ -485,7 +520,8 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sbi
         const int nvalid = LEAN ? 32 : min(ncols, p.Cout - n0);
         const bool live = valid && nvalid > 0;
         const long long off = pix_off + n0;
-        const bool vec = !f32out && live && (nvalid == ncols) && ((off & 7) == 0);
+        // 16-byte accesses: the hi address and, in the (hi, lo) layout, the lo plane `out_lo` elements further
+        const bool vec = !f32out && live && (nvalid == ncols) && ((off & 7) == 0) && ((out_lo & 7) == 0);
         // operands that do not depend on the accumulator are fetched BEFORE waiting on it
         float bz[32];
         bias32(sbias, n_base - bias_origin + c0, bz);

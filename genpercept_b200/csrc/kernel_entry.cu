@@ -76,6 +76,14 @@ void fill_attention_operands(bool bf16, void* qk, size_t qk_n, void* vT, size_t 
                          cudaMemcpyHostToDevice));
 }
 
+// The storage layout of a per-kernel call: GP_F16 / GP_BF16, or (where the entry point takes it) GP_F16_PAIR, the
+// high-precision mode's [hi C | lo C] fp16 pairs.  Returns true for the pair layout.
+bool storage_layout(int dtype, bool pair_ok, const char* fn) {
+  GP_REQUIRE(dtype == GP_F16 || dtype == GP_BF16 || (pair_ok && dtype == GP_F16_PAIR),
+             std::string(fn) + (pair_ok ? ": dtype must be f16, bf16 or f16 pair" : ": dtype must be f16/bf16"));
+  return dtype == GP_F16_PAIR;
+}
+
 }  // namespace
 
 extern "C" {
@@ -84,13 +92,13 @@ gp_status gp_conv2d(int dtype, const void* x, int N, int H, int W, int Cin, cons
                     int Cout, int ks, int mode, const void* residual, int relu, void* y, int use_direct, void* stream) {
   return guarded_free([&]() {
     GP_REQUIRE(x && w_host && y && (ks == 1 || ks == 3) && mode >= 0 && mode <= 3, "gp_conv2d: bad arguments");
-    GP_REQUIRE(dtype == GP_F16 || dtype == GP_BF16, "gp_conv2d: dtype must be f16/bf16");
+    const bool pair = storage_layout(dtype, true, "gp_conv2d");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    WeightStore ws(dtype == GP_BF16);
+    WeightStore ws(dtype == GP_BF16, pair);
     ws.put("t.weight", {Cout, Cin, ks, ks}, w_host);
     if (bias_host) ws.put("t.bias", {Cout}, bias_host);
     const auto [Ho, Wo] = conv_out_dims(mode, H, W);
-    Builder b(ws.bf16, false, nullptr);
+    Builder b(ws.bf16, false, nullptr, ws.split);
     T4 xin = b.external(x, N, H, W, Cin);
     T4 yout = b.external(y, N, Ho, Wo, Cout);
     T4 res;
@@ -99,9 +107,9 @@ gp_status gp_conv2d(int dtype, const void* x, int N, int H, int W, int Cin, cons
       const DirectW& dw = ws.direct_w("t", Cin);
       DirectConvParams p;
       std::memset(&p, 0, sizeof(p));
-      p.in = x; p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.in_cstride = Cin;
+      p.in = x; p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.in_cstride = (int)xin.ps(); p.in_lo = pair ? Cin : 0;
       p.w = dw.w; p.bias = dw.bias; p.res = residual;
-      p.out = y; p.Ho = Ho; p.Wo = Wo; p.Cout = Cout; p.out_cstride = Cout;
+      p.out = y; p.Ho = Ho; p.Wo = Wo; p.Cout = Cout; p.out_cstride = (int)yout.ps(); p.out_lo = pair ? Cout : 0;
       p.ks = ks;
       p.stride = (mode == 1 || mode == 2) ? 2 : 1;
       p.pad = (mode == 2) ? 0 : ks / 2;
@@ -132,8 +140,10 @@ gp_status gp_conv2d(int dtype, const void* x, int N, int H, int W, int Cin, cons
 gp_status gp_groupnorm(int dtype, const void* x, int N, int H, int W, int C, int groups, const float* gamma_host,
                        const float* beta_host, float eps, int silu, void* y, void* stream) {
   return guarded_free([&]() {
+    GP_REQUIRE(x && y && gamma_host && beta_host && groups >= 1 && C % groups == 0 && C % 8 == 0, "gp_groupnorm: bad arguments");
+    const bool pair = storage_layout(dtype, true, "gp_groupnorm");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    WeightStore ws(dtype == GP_BF16);
+    WeightStore ws(dtype == GP_BF16, pair);
     ws.put("gn.weight", {C}, gamma_host);
     ws.put("gn.bias", {C}, beta_host);
     const NormW& nw = ws.norm_w("gn");
@@ -151,9 +161,9 @@ gp_status gp_gn_conv3x3(int dtype, const void* x, int N, int H, int W, int Cin, 
                         void* y, int out_f32, void* stream) {
   return guarded_free([&]() {
     GP_REQUIRE(x && w_host && y && gamma_host && beta_host, "gp_gn_conv3x3: bad arguments");
-    GP_REQUIRE(dtype == GP_F16 || dtype == GP_BF16, "gp_gn_conv3x3: dtype must be f16/bf16");
+    const bool pair = storage_layout(dtype, true, "gp_gn_conv3x3");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    WeightStore ws(dtype == GP_BF16);
+    WeightStore ws(dtype == GP_BF16, pair);
     ws.put("t.weight", {Cout, Cin, 3, 3}, w_host);
     std::vector<float> zb(Cout, 0.f);
     ws.put("t.bias", {Cout}, bias_host ? bias_host : zb.data());
@@ -183,14 +193,50 @@ gp_status gp_gn_conv3x3(int dtype, const void* x, int N, int H, int W, int Cin, 
   });
 }
 
+gp_status gp_conv_groupnorm(int dtype, const void* x, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
+                            int Cout, const void* skip, int Cskip, int groups, const float* gamma_host, const float* beta_host,
+                            float eps, int silu, void* y_conv, void* y, void* stream) {
+  return guarded_free([&]() {
+    GP_REQUIRE(x && w_host && y_conv && y && gamma_host && beta_host && groups >= 1 && Cout % 8 == 0 && Cskip % 8 == 0 &&
+                   (skip ? Cskip > 0 : Cskip == 0) && (Cout + Cskip) % groups == 0,
+               "gp_conv_groupnorm: bad arguments");
+    const bool pair = storage_layout(dtype, true, "gp_conv_groupnorm");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    WeightStore ws(dtype == GP_BF16, pair);
+    ws.put("t.weight", {Cout, Cin, 3, 3}, w_host);
+    std::vector<float> zb(Cout, 0.f);
+    ws.put("t.bias", {Cout}, bias_host ? bias_host : zb.data());
+    const int Ctot = Cout + Cskip;
+    ws.put("gn.weight", {Ctot}, gamma_host);
+    ws.put("gn.bias", {Ctot}, beta_host);
+    const NormW& nw = ws.norm_w("gn");
+    float* ss = ws.upload(std::vector<float>((size_t)N * Ctot * 2, 0.f));
+    const PackedW& pw = ws.conv_w("t", {Cin});
+    build_and_run(ws, s, [&](Builder& b) {
+      b.gn_ss = ss;
+      ConvArgs c;
+      c.srcs = {b.external(x, N, H, W, Cin)};
+      c.w = &pw;
+      c.out = b.external(y_conv, N, H, W, Cout);
+      c.want_stats = true;
+      b.conv("gp_conv_groupnorm.conv", c);
+      std::vector<T4> srcs = {c.out};
+      if (skip) srcs.push_back(b.external(skip, N, H, W, Cskip));
+      b.gn("gp_conv_groupnorm.gn", srcs, nw, groups, eps, silu != 0, b.external(y, N, H, W, Ctot));
+    });
+  });
+}
+
 gp_status gp_layernorm(int dtype, const void* x, int64_t tokens, int C, const float* gamma_host, const float* beta_host,
                        float eps, void* y, void* stream) {
   return guarded_free([&]() {
+    GP_REQUIRE(x && y && gamma_host && beta_host && tokens >= 0 && C >= 8, "gp_layernorm: bad arguments");
+    const bool pair = storage_layout(dtype, true, "gp_layernorm");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    WeightStore ws(dtype == GP_BF16);
+    WeightStore ws(dtype == GP_BF16, pair);
     float* g = ws.upload(std::vector<float>(gamma_host, gamma_host + C));
     float* bt = ws.upload(std::vector<float>(beta_host, beta_host + C));
-    GP_CUDA(layernorm(x, y, tokens, C, g, bt, eps, ws.bf16, s));
+    GP_CUDA(layernorm(x, y, tokens, C, g, bt, eps, ws.bf16, s, pair));
     GP_CUDA(cudaStreamSynchronize(s));
   });
 }
@@ -201,6 +247,7 @@ gp_status gp_attention(int dtype, const void* q, const void* k, const void* v, i
     // q is pre-scaled by the caller-visible `scale` through an identity-weight GEMM, and V^T is the engine's own
     // swapped-operand GEMM with identity weights, so that the same igemm paths the engine uses (QK^T, softmax, V^T, PV)
     // are exercised.
+    storage_layout(dtype, false, "gp_attention");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     WeightStore ws(dtype == GP_BF16);
     const int C = heads * d;
@@ -264,8 +311,10 @@ gp_status gp_ensemble_reduce(const float* pred_dev, int B, int H, int W, const f
 
 gp_status gp_bilinear_up2x(int dtype, const void* x, int N, int H, int W, int C, void* y, void* stream) {
   return guarded_free([&]() {
+    GP_REQUIRE(x && y && N >= 1 && H >= 1 && W >= 1 && C >= 1, "gp_bilinear_up2x: bad arguments");
+    const bool pair = storage_layout(dtype, true, "gp_bilinear_up2x");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    GP_CUDA(bilinear_up2x(x, y, N, H, W, C, dtype == GP_BF16, s));
+    GP_CUDA(bilinear_up2x(x, y, N, H, W, C, dtype == GP_BF16, s, pair));
     GP_CUDA(cudaStreamSynchronize(s));
   });
 }
@@ -273,6 +322,7 @@ gp_status gp_bilinear_up2x(int dtype, const void* x, int N, int H, int W, int C,
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters, double* usec,
                         double* flops) {
   return guarded_free([&]() {
+    storage_layout(dtype, false, "gp_bench_conv");
     WeightStore ws(dtype == GP_BF16);
     const std::vector<float> wt((size_t)Cout * Cin * ks * ks, 0.01f), bz(Cout, 0.f);
     ws.put("t.weight", {Cout, Cin, ks, ks}, wt.data());
@@ -297,7 +347,7 @@ gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int k
 
 gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, double* usec, double* flops) {
   return guarded_free([&]() {
-    GP_REQUIRE(dtype == GP_F16 || dtype == GP_BF16, "gp_bench_attention: dtype must be f16/bf16");
+    storage_layout(dtype, false, "gp_bench_attention");
     GP_REQUIRE(B >= 1 && T >= 1 && iters >= 1, "gp_bench_attention: bad arguments");
     WeightStore ws(dtype == GP_BF16);
     const int C = 512;

@@ -134,68 +134,77 @@ __global__ void direct_conv_kernel(const DirectConvParams p) {
 }
 
 // ------------------------------------------------------------------------------ GroupNorm
-// Deterministic two-level reduction (no atomics, fixed summation order => bit-reproducible runs):
-//   gn_stats   : block (C/8 vectors x PIX pixel lanes) reduces its pixel chunk -> partial[n][chunk][c][2]
-//   gn_finalize: one warp per (n, group) sums the partials in a fixed order -> scale/shift per channel
+// Deterministic two-level reduction (no atomics, fixed merge order => bit-reproducible runs) of (count, mean, M2)
+// records (kernels.h):
+//   gn_stats   : each thread sums its pixels as deviations from the first of them; the block merges its pixel lanes
+//                -> partial[n][chunk][c][kGnRec]
+//   gn_finalize: one CTA per (n, group) merges the partials in a fixed order -> scale/shift per channel
 template <bool BF16>
 __global__ void gn_stats_kernel(const uint16_t* __restrict__ x, long long HW, int C, float* __restrict__ partial,
                                 int Ctot, int coff, int pix_per_block, int xs, int lo) {
-  extern __shared__ float sh[];   // [PIX][C][2]
+  extern __shared__ float sh[];   // [PIX][C][2] (mean, M2), then [PIX] counts
+  float* shn = sh + (size_t)blockDim.y * C * 2;
   const int n = blockIdx.y;
   const int tid = threadIdx.y * blockDim.x + threadIdx.x;
   const int nthr = blockDim.x * blockDim.y;
   const long long p0 = (long long)blockIdx.x * pix_per_block;
   long long p1 = p0 + pix_per_block;
   if (p1 > HW) p1 = HW;
-  float s[8], q[8];
+  float k[8], s[8], q[8];
 #pragma unroll
-  for (int e = 0; e < 8; ++e) { s[e] = 0.f; q[e] = 0.f; }
+  for (int e = 0; e < 8; ++e) { k[e] = 0.f; s[e] = 0.f; q[e] = 0.f; }
   const uint16_t* base = x + ((long long)n * HW) * xs + threadIdx.x * 8;
   const int step = blockDim.y;
   long long p = p0 + threadIdx.y;
+  if (p < p1) load8<BF16>(base + p * xs, lo, k);      // the shift: this thread's first pixel
+  const long long first = p;
   for (; p + 3 * step < p1 && !lo; p += 4 * step) {      // four independent 16-byte loads in flight
     uint4 u[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) u[k] = __ldg(reinterpret_cast<const uint4*>(base + (p + (long long)k * step) * xs));
+    for (int kk = 0; kk < 4; ++kk) u[kk] = __ldg(reinterpret_cast<const uint4*>(base + (p + (long long)kk * step) * xs));
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
+    for (int kk = 0; kk < 4; ++kk) {
       float f[8];
-      unpack8<BF16>(u[k], f);
+      unpack8<BF16>(u[kk], f);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) { s[e] += f[e]; q[e] += f[e] * f[e]; }
+      for (int e = 0; e < 8; ++e) { const float d = f[e] - k[e]; s[e] += d; q[e] = fmaf(d, d, q[e]); }
     }
   }
   for (; p < p1; p += step) {
     float f[8];
     load8<BF16>(base + p * xs, lo, f);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { s[e] += f[e]; q[e] += f[e] * f[e]; }
+    for (int e = 0; e < 8; ++e) { const float d = f[e] - k[e]; s[e] += d; q[e] = fmaf(d, d, q[e]); }
   }
+  const long long cnt_ll = first < p1 ? (p1 - 1 - first) / step + 1 : 0;
+  const float cnt = (float)cnt_ll, inv = cnt_ll ? 1.f / cnt : 0.f;
   float* mine = sh + ((size_t)threadIdx.y * C + threadIdx.x * 8) * 2;
 #pragma unroll
-  for (int e = 0; e < 8; ++e) { mine[2 * e] = s[e]; mine[2 * e + 1] = q[e]; }
+  for (int e = 0; e < 8; ++e) { mine[2 * e] = fmaf(s[e], inv, k[e]); mine[2 * e + 1] = fmaxf(q[e] - s[e] * s[e] * inv, 0.f); }
+  if (threadIdx.x == 0) shn[threadIdx.y] = cnt;
   __syncthreads();
-  float* dst = partial + (((long long)n * gridDim.x + blockIdx.x) * Ctot + coff) * 2;
-  for (int i = tid; i < 2 * C; i += nthr) {
-    float a = 0.f;
-    for (int y = 0; y < (int)blockDim.y; ++y) a += sh[(size_t)y * C * 2 + i];
-    dst[i] = a;
+  float* dst = partial + (((long long)n * gridDim.x + blockIdx.x) * Ctot + coff) * kGnRec;
+  for (int c = tid; c < C; c += nthr) {
+    float rn = 0.f, rm = 0.f, r2 = 0.f;
+    for (int y = 0; y < (int)blockDim.y; ++y)
+      chan_merge(rn, rm, r2, shn[y], sh[((size_t)y * C + c) * 2], sh[((size_t)y * C + c) * 2 + 1]);
+    dst[c * kGnRec] = rn; dst[c * kGnRec + 1] = rm; dst[c * kGnRec + 2] = r2;
   }
 }
 
-// One CTA of 256 threads per (image, group): the partial sums (one slot per producing CTA or pixel chunk, up to
-// 256 x channels-per-group entries) are read with all 8 warps in flight and reduced in a fixed order (thread ->
-// warp shuffle -> 8 warp totals), so the result does not depend on scheduling.  (One WARP per group would leave the
+// One CTA of 256 threads per (image, group): the partials (one slot per producing CTA or pixel chunk, up to
+// 256 x channels-per-group entries) are read with all 8 warps in flight and merged in a fixed order (thread ->
+// warp shuffle tree -> 8 warp records), so the result does not depend on scheduling.  (One WARP per group would leave the
 // kernel latency-bound on the few SMs that have a group.)
 __global__ void __launch_bounds__(256) gn_finalize_kernel(GnSrc s0, GnSrc s1, int nsrc, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, int N, int Ctot, int groups,
                                                           float inv_count, float eps, float* __restrict__ ss) {
-  __shared__ float red[2][8];
+  __shared__ float red[3][8];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x / groups, g = blockIdx.x % groups;
   const int cpg = Ctot / groups;
   const int glo = g * cpg, ghi = glo + cpg;
-  float s = 0.f, q = 0.f;
+  float rn = 0.f, rm = 0.f, r2 = 0.f;
   int cbase = 0;
   for (int si = 0; si < nsrc; ++si) {
     const GnSrc src = si == 0 ? s0 : s1;
@@ -205,25 +214,30 @@ __global__ void __launch_bounds__(256) gn_finalize_kernel(GnSrc s0, GnSrc s1, in
       const int entries = w * src.chunks;
       for (int i = threadIdx.x; i < entries; i += 256) {
         const int ch = i / w, c = lo - cbase + (i - ch * w);
-        const float2 v = *reinterpret_cast<const float2*>(src.partial + (((long long)n * src.chunks + ch) * src.C + c) * 2);
-        s += v.x; q += v.y;
+        const float* v = src.partial + (((long long)n * src.chunks + ch) * src.C + c) * kGnRec;
+        chan_merge(rn, rm, r2, v[0], v[1], v[2]);
       }
     }
     cbase += src.C;
   }
-  s = warp_sum(s); q = warp_sum(q);
-  if (lane == 0) { red[0][warp] = s; red[1][warp] = q; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float bn = __shfl_xor_sync(0xffffffffu, rn, o), bm = __shfl_xor_sync(0xffffffffu, rm, o),
+                b2 = __shfl_xor_sync(0xffffffffu, r2, o);
+    chan_merge(rn, rm, r2, bn, bm, b2);
+  }
+  if (lane == 0) { red[0][warp] = rn; red[1][warp] = rm; red[2][warp] = r2; }
   __syncthreads();
-  s = ((red[0][0] + red[0][1]) + (red[0][2] + red[0][3])) + ((red[0][4] + red[0][5]) + (red[0][6] + red[0][7]));
-  q = ((red[1][0] + red[1][1]) + (red[1][2] + red[1][3])) + ((red[1][4] + red[1][5]) + (red[1][6] + red[1][7]));
-  const float mean = s * inv_count;
-  const float var = fmaxf(q * inv_count - mean * mean, 0.f);
+  rn = red[0][0]; rm = red[1][0]; r2 = red[2][0];
+  for (int w = 1; w < 8; ++w) chan_merge(rn, rm, r2, red[0][w], red[1][w], red[2][w]);
+  const float mean = rm;
+  const float var = r2 * inv_count;
   const float rstd = rsqrtf(var + eps);
   for (int i = threadIdx.x; i < cpg; i += 256) {
     const int c = glo + i;
     const float sc = rstd * gamma[c];
     ss[((long long)n * Ctot + c) * 2] = sc;
-    ss[((long long)n * Ctot + c) * 2 + 1] = beta[c] - mean * sc;
+    ss[((long long)n * Ctot + c) * 2 + 1] = fmaf(-mean, sc, beta[c]);
   }
 }
 
@@ -910,7 +924,7 @@ cudaError_t gn_stats(const void* x, int N, long long HW, int C, float* partial, 
   const int pix_per_block = (int)((HW + chunks - 1) / chunks);
   dim3 block(nvec, pix);
   dim3 grid((unsigned)chunks, N);
-  const size_t smem = (size_t)pix * C * 2 * sizeof(float);
+  const size_t smem = ((size_t)pix * C * 2 + pix) * sizeof(float);
   GP_DISPATCH_BF16(bf16, (launch(gn_stats_kernel<BF>, grid, block, smem, s, reinterpret_cast<const uint16_t*>(x), HW, C,
                                                                          partial, Ctot, coff, pix_per_block,
                                                                          split ? 2 * C : C, split ? C : 0)));

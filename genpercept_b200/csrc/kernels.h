@@ -30,14 +30,31 @@ struct DirectConvParams {
 };
 cudaError_t direct_conv(const DirectConvParams& p, bool bf16, cudaStream_t s);
 
-// GroupNorm, deterministic: per-chunk partial sums [N][chunks][Ctot][2] -> per-(n, channel)
+// GroupNorm, deterministic: per-chunk partials [N][chunks][Ctot][kGnRec] -> per-(n, channel)
 // scale / shift -> apply.  chunks = gn_chunks(N, HW) for every source of one normalisation.
+// A partial is (count, mean, M2) of one channel over its pixels, M2 = sum of squared deviations from that mean:
+// the variance stays accurate at any mean / std ratio, where sum / sum-of-squares cancels.  A record of count 0
+// (an untouched, zeroed slot) merges as nothing.
+constexpr int kGnRec = 3;
 int gn_chunks(int N, long long HW);
 cudaError_t gn_stats(const void* x, int N, long long HW, int C, float* partial, int chunks, int Ctot, int coff,
                      bool bf16, cudaStream_t s, bool split = false);
-// one source of a (possibly concatenated) normalisation: partial sums [N][chunks][C][2]; the partials
+// one source of a (possibly concatenated) normalisation: partials [N][chunks][C][kGnRec]; the partials
 // come either from gn_stats or from the producing implicit-GEMM's epilogue (IgemmParams::stats).
 struct GnSrc { const float* partial; int chunks; int C; };
+
+#ifdef __CUDACC__
+// Chan et al.'s pairwise update: (na, ma, m2a) <- the statistics of the union of a and (nb, mb, m2b).  The weight
+// nb / n takes the fast division (2 ulp; an IEEE division is a called slow path, which costs the GEMM epilogue spills).
+__device__ __forceinline__ void chan_merge(float& na, float& ma, float& m2a, float nb, float mb, float m2b) {
+  const float n = na + nb;
+  const float f = n > 0.f ? __fdividef(nb, n) : 0.f;
+  const float d = mb - ma;
+  ma = fmaf(d, f, ma);
+  m2a = m2a + m2b + d * d * na * f;
+  na = n;
+}
+#endif
 cudaError_t gn_finalize(const GnSrc* srcs, int nsrc, const float* gamma, const float* beta, int N, int Ctot,
                         int groups, long long HW, float eps, float* scale_shift /*[N][Ctot][2]*/, cudaStream_t s);
 cudaError_t gn_apply(const void* x, int N, long long HW, int C, const float* scale_shift, int Ctot,

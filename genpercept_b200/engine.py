@@ -14,7 +14,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgenpercept_b200.so")
 
-GP_F32, GP_F16, GP_BF16, GP_U8 = 0, 1, 2, 3
+GP_F32, GP_F16, GP_BF16, GP_U8, GP_F16_PAIR = 0, 1, 2, 3, 4
 GP_READOUT_VAE, GP_READOUT_DPT = 0, 1
 STAGE_PRE, STAGE_VAE_ENCODE, STAGE_UNET, STAGE_READOUT = 0, 1, 2, 3
 _STATUS = {0: "GP_OK", 1: "GP_ERR_INVALID", 2: "GP_ERR_MISSING", 3: "GP_ERR_NO_PLAN", 4: "GP_ERR_CUDA",
@@ -78,6 +78,8 @@ def lib():
     L.gp_gn_conv3x3.argtypes = [c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int,
                                 c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                 c_void_p]
+    L.gp_conv_groupnorm.argtypes = [c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                    c_int, c_void_p, c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p]
     L.gp_layernorm.argtypes = [c_int, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p]
     L.gp_attention.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                c_void_p]
@@ -366,13 +368,49 @@ def shared_arena_fill(byte, device=0):
 
 
 # ---------------------------------------------------------------- per-kernel entry points (tests)
+# An fp32 activation selects the high-precision mode's layout (GP_F16_PAIR): it is split into its (hi, lo) fp16 pair,
+# stored [hi C | lo C] per pixel, and the result comes back as float64 hi + lo, the exact stored value (an fp32 sum is not
+# exact where lo is far below hi's last bit).  f16 / bf16 activations run the 16-bit modes and come back as they are.
 def _nhwc(x):
     """NCHW torch tensor -> contiguous NHWC (same dtype)."""
     return x.permute(0, 2, 3, 1).contiguous()
 
 
+def _layout(x):
+    """The C-ABI dtype of a per-kernel call on activation `x`."""
+    return GP_F16_PAIR if x.dtype == torch.float32 else _gp_dtype(x.dtype)
+
+
+def _arg(t, dt):
+    """Activation `t` (or None) as the kernels take it in layout `dt`: contiguous, fp32 split into [hi | lo] channels."""
+    if t is None:
+        return None
+    if dt == GP_F16_PAIR:
+        assert t.dtype == torch.float32, "every activation of a high-precision call is fp32"
+        return torch.cat(split_hi_lo(t), dim=-1).contiguous()
+    assert t.dtype != torch.float32, "fp32 activations select the high-precision layout for every operand"
+    return t.contiguous()
+
+
+def _out(shape, dt, device):
+    """An output buffer of logical `shape` (channels last) in layout `dt`."""
+    if dt == GP_F16_PAIR:
+        return torch.zeros(tuple(shape[:-1]) + (2 * shape[-1],), dtype=torch.float16, device=device)
+    return torch.zeros(tuple(shape), dtype=torch.bfloat16 if dt == GP_BF16 else torch.float16, device=device)
+
+
+def _result(y, dt):
+    """An output buffer as the caller sees it: float64 hi + lo in the pair layout."""
+    if dt == GP_F16_PAIR:
+        c = y.shape[-1] // 2
+        return y[..., :c].double() + y[..., c:].double()
+    return y
+
+
 def conv2d(x_nhwc, w, bias=None, mode=0, residual=None, relu=False, direct=False):
-    """x_nhwc: cuda [N,H,W,Cin] f16/bf16; w: cpu fp32 [Cout,Cin,ks,ks]. Returns NHWC."""
+    """x_nhwc: cuda [N,H,W,Cin] f16/bf16, or fp32 (the (hi, lo) pair layout); w: cpu fp32 [Cout,Cin,ks,ks]. Returns NHWC
+    (float64 for an fp32 input)."""
+    dt = _layout(x_nhwc)
     N, H, W, Cin = x_nhwc.shape
     Cout, _, ks, _ = w.shape
     Ho, Wo = H, W
@@ -382,46 +420,68 @@ def conv2d(x_nhwc, w, bias=None, mode=0, residual=None, relu=False, direct=False
         Ho, Wo = (H + 1 - 3) // 2 + 1, (W + 1 - 3) // 2 + 1
     elif mode == 3:
         Ho, Wo = 2 * H, 2 * W
-    y = torch.zeros((N, Ho, Wo, Cout), dtype=x_nhwc.dtype, device=x_nhwc.device)
+    y = _out((N, Ho, Wo, Cout), dt, x_nhwc.device)
+    x, res = _arg(x_nhwc, dt), _arg(residual, dt)
     w = w.detach().float().cpu().contiguous()
     b = bias.detach().float().cpu().contiguous() if bias is not None else None
-    st = lib().gp_conv2d(_gp_dtype(x_nhwc.dtype), c_void_p(x_nhwc.data_ptr()), N, H, W, Cin, c_void_p(w.data_ptr()),
-                         c_void_p(b.data_ptr()) if b is not None else None, Cout, ks, mode,
-                         c_void_p(residual.data_ptr()) if residual is not None else None, 1 if relu else 0,
+    st = lib().gp_conv2d(dt, c_void_p(x.data_ptr()), N, H, W, Cin, c_void_p(w.data_ptr()),
+                         c_void_p(b.data_ptr()) if b is not None else None, Cout, ks, mode, _ptr(res), 1 if relu else 0,
                          c_void_p(y.data_ptr()), 1 if direct else 0, _stream_ptr())
     _check_free(st, "gp_conv2d")
-    return y
+    return _result(y, dt)
 
 
 def groupnorm(x_nhwc, groups, gamma, beta, eps, silu):
+    """GroupNorm(+SiLU) on NHWC x (f16/bf16, or fp32: the pair layout, float64 result)."""
+    dt = _layout(x_nhwc)
     N, H, W, C = x_nhwc.shape
-    y = torch.empty_like(x_nhwc)
+    x = _arg(x_nhwc, dt)
+    y = _out((N, H, W, C), dt, x_nhwc.device)
     g = gamma.detach().float().cpu().contiguous()
     b = beta.detach().float().cpu().contiguous()
-    st = lib().gp_groupnorm(_gp_dtype(x_nhwc.dtype), c_void_p(x_nhwc.data_ptr()), N, H, W, C, groups,
-                            c_void_p(g.data_ptr()), c_void_p(b.data_ptr()), eps, 1 if silu else 0,
-                            c_void_p(y.data_ptr()), _stream_ptr())
+    st = lib().gp_groupnorm(dt, c_void_p(x.data_ptr()), N, H, W, C, groups, c_void_p(g.data_ptr()), c_void_p(b.data_ptr()),
+                            eps, 1 if silu else 0, c_void_p(y.data_ptr()), _stream_ptr())
     _check_free(st, "gp_groupnorm")
-    return y
+    return _result(y, dt)
 
 
 def gn_conv3x3(x_nhwc, groups, gamma, beta, eps, silu, w, bias=None, sc_x=None, sc_w=None, sc_b=None, residual=None,
                out_f32=False):
-    """GroupNorm(+SiLU) -> 3x3 conv (+ 1x1 shortcut over raw sc_x, + residual) through gp_gn_conv3x3."""
+    """GroupNorm(+SiLU) -> 3x3 conv (+ 1x1 shortcut over raw sc_x, + residual) through gp_gn_conv3x3.  An fp32 x selects
+    the pair layout (sc_x and residual fp32 too) and a float64 NHWC result; out_f32: an fp32 NCHW map either way."""
+    dt = _layout(x_nhwc)
     N, H, W, Cin = x_nhwc.shape
     Cout = w.shape[0]
     f = lambda t: None if t is None else t.detach().float().cpu().contiguous()
     g, b_, w_, bias_, scw, scb = f(gamma), f(beta), f(w), f(bias), f(sc_w), f(sc_b)
-    pp = lambda t: None if t is None else c_void_p(t.data_ptr())
+    x, scx, res = _arg(x_nhwc, dt), _arg(sc_x, dt), _arg(residual, dt)
     if out_f32:
         y = torch.zeros((N, Cout, H, W), dtype=torch.float32, device=x_nhwc.device)
     else:
-        y = torch.zeros((N, H, W, Cout), dtype=x_nhwc.dtype, device=x_nhwc.device)
-    st = lib().gp_gn_conv3x3(_gp_dtype(x_nhwc.dtype), pp(x_nhwc), N, H, W, Cin, groups, pp(g), pp(b_), eps, 1 if silu else 0,
-                             pp(w_), pp(bias_), Cout, pp(sc_x), 0 if sc_x is None else sc_x.shape[-1], pp(scw), pp(scb),
-                             pp(residual), pp(y), 1 if out_f32 else 0, _stream_ptr())
+        y = _out((N, H, W, Cout), dt, x_nhwc.device)
+    st = lib().gp_gn_conv3x3(dt, _ptr(x), N, H, W, Cin, groups, _ptr(g), _ptr(b_), eps, 1 if silu else 0,
+                             _ptr(w_), _ptr(bias_), Cout, _ptr(scx), 0 if sc_x is None else sc_x.shape[-1], _ptr(scw), _ptr(scb),
+                             _ptr(res), _ptr(y), 1 if out_f32 else 0, _stream_ptr())
     _check_free(st, "gp_gn_conv3x3")
-    return y
+    return y if out_f32 else _result(y, dt)
+
+
+def conv_groupnorm(x_nhwc, w, bias, groups, gamma, beta, eps, silu, skip=None):
+    """3x3 stride-1 conv x -> y_conv, then GroupNorm(+SiLU) over concat(y_conv, skip) -> y (gp_conv_groupnorm).  Returns
+    (y_conv, y) NHWC; an fp32 x (and skip) selects the pair layout and float64 results."""
+    dt = _layout(x_nhwc)
+    N, H, W, Cin = x_nhwc.shape
+    Cout = w.shape[0]
+    Cskip = 0 if skip is None else skip.shape[-1]
+    f = lambda t: None if t is None else t.detach().float().cpu().contiguous()
+    w_, b_, g, bt = f(w), f(bias), f(gamma), f(beta)
+    x, sk = _arg(x_nhwc, dt), _arg(skip, dt)
+    yc = _out((N, H, W, Cout), dt, x_nhwc.device)
+    y = _out((N, H, W, Cout + Cskip), dt, x_nhwc.device)
+    st = lib().gp_conv_groupnorm(dt, _ptr(x), N, H, W, Cin, _ptr(w_), _ptr(b_), Cout, _ptr(sk), Cskip, groups, _ptr(g), _ptr(bt),
+                                 eps, 1 if silu else 0, _ptr(yc), _ptr(y), _stream_ptr())
+    _check_free(st, "gp_conv_groupnorm")
+    return _result(yc, dt), _result(y, dt)
 
 
 def ensemble_reduce(pred, scale, shift, median=True, normalise=1):
@@ -439,14 +499,17 @@ def ensemble_reduce(pred, scale, shift, median=True, normalise=1):
 
 
 def layernorm(x, gamma, beta, eps=1e-5):
+    """LayerNorm over the last axis of cuda x (f16/bf16, or fp32: the pair layout, float64 result)."""
+    dt = _layout(x)
     C = x.shape[-1]
-    y = torch.empty_like(x)
+    xa = _arg(x, dt)
+    y = _out(tuple(x.shape), dt, x.device)
     g = gamma.detach().float().cpu().contiguous()
     b = beta.detach().float().cpu().contiguous()
-    st = lib().gp_layernorm(_gp_dtype(x.dtype), c_void_p(x.data_ptr()), x.numel() // C, C, c_void_p(g.data_ptr()),
+    st = lib().gp_layernorm(dt, c_void_p(xa.data_ptr()), x.numel() // C, C, c_void_p(g.data_ptr()),
                             c_void_p(b.data_ptr()), eps, c_void_p(y.data_ptr()), _stream_ptr())
     _check_free(st, "gp_layernorm")
-    return y
+    return _result(y, dt)
 
 
 def attention(q, k, v, heads, scale):
@@ -483,12 +546,14 @@ def attention_high(q, k, v, heads, scale, fused):
 
 
 def bilinear_up2x(x_nhwc):
+    """Bilinear 2x (align_corners=True) on NHWC x (f16/bf16, or fp32: the pair layout, float64 result)."""
+    dt = _layout(x_nhwc)
     N, H, W, C = x_nhwc.shape
-    y = torch.empty((N, 2 * H, 2 * W, C), dtype=x_nhwc.dtype, device=x_nhwc.device)
-    st = lib().gp_bilinear_up2x(_gp_dtype(x_nhwc.dtype), c_void_p(x_nhwc.data_ptr()), N, H, W, C,
-                                c_void_p(y.data_ptr()), _stream_ptr())
+    x = _arg(x_nhwc, dt)
+    y = _out((N, 2 * H, 2 * W, C), dt, x_nhwc.device)
+    st = lib().gp_bilinear_up2x(dt, c_void_p(x.data_ptr()), N, H, W, C, c_void_p(y.data_ptr()), _stream_ptr())
     _check_free(st, "gp_bilinear_up2x")
-    return y
+    return _result(y, dt)
 
 
 RESIZE_MODES = {"bilinear": 0, "bicubic": 1}

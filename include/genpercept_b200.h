@@ -34,7 +34,10 @@ typedef enum {
   GP_ERR_STATE = 5      /* call order (e.g. gp_plan before gp_finalize)                     */
 } gp_status;
 
-typedef enum { GP_F32 = 0, GP_F16 = 1, GP_BF16 = 2, GP_U8 = 3 } gp_dtype;
+/* GP_F16_PAIR: the high-precision mode's storage layout (gp_config.precision = 1), taken by the per-kernel entry points
+ * that say so: a 16-bit tensor of C logical channels carries [hi C | lo C] fp16 per pixel, value = hi + lo.  Every other
+ * entry point rejects it with GP_ERR_INVALID. */
+typedef enum { GP_F32 = 0, GP_F16 = 1, GP_BF16 = 2, GP_U8 = 3, GP_F16_PAIR = 4 } gp_dtype;
 typedef enum { GP_READOUT_VAE = 0, GP_READOUT_DPT = 1 } gp_readout;
 
 typedef struct {
@@ -180,10 +183,15 @@ gp_status gp_profile_ops(gp_engine* e, int out_channels, void* stream);
 gp_status gp_op_info(gp_engine* e, int64_t i, char* name_buf, size_t name_cap, double* usec, double* flops,
                      double* bytes, int* kind, double* flops_exec);
 
-/* ---- per-kernel entry points (parity tests, micro-benchmarks); all pointers are device ---- */
+/* ---- per-kernel entry points (parity tests, micro-benchmarks); all pointers are device ----
+ * dtype: GP_F16 or GP_BF16; gp_conv2d, gp_groupnorm, gp_gn_conv3x3, gp_conv_groupnorm, gp_layernorm and
+ * gp_bilinear_up2x also take GP_F16_PAIR, in which every 16-bit tensor (inputs, residual, skip, shortcut, outputs) has
+ * the [hi C | lo C] layout and the contractions run the high-precision mode's three passes (hi*hi + lo*hi + hi*lo). */
 /* 3x3 / 1x1 convolution through the wgmma implicit-GEMM kernels.  x: 16-bit NHWC [N,H,W,Cin];
  * w: fp32 [Cout,Cin,ks,ks] (host); mode: 0 stride-1 pad ks/2, 1 stride-2 pad (1,1,1,1),
- * 2 stride-2 pad (0,1,0,1) (VAE encoder), 3 nearest-2x upsample then stride-1.  y: 16-bit NHWC. */
+ * 2 stride-2 pad (0,1,0,1) (VAE encoder), 3 nearest-2x upsample then stride-1.  y: 16-bit NHWC.
+ * GP_F16_PAIR through the implicit GEMM needs Cin % 8 == 0 (the lo plane of a pixel must start 16-byte aligned);
+ * use_direct_kernel takes any Cin. */
 gp_status gp_conv2d(int dtype, const void* x, int N, int H, int W, int Cin, const float* w_host,
                     const float* bias_host, int Cout, int ks, int mode, const void* residual, int relu,
                     void* y, int use_direct_kernel, void* stream);
@@ -198,6 +206,14 @@ gp_status gp_gn_conv3x3(int dtype, const void* x, int N, int H, int W, int Cin, 
                         const float* beta_host, float eps, int silu, const float* w_host, const float* bias_host, int Cout,
                         const void* sc_x, int Csc, const float* sc_w_host, const float* sc_b_host, const void* residual,
                         void* y, int out_f32, void* stream);
+/* 3x3 stride-1 convolution x [N,H,W,Cin] -> y_conv [N,H,W,Cout] (16-bit NHWC, bias optional), then GroupNorm(groups,
+ * eps)(+SiLU) over concat(y_conv, skip) -> y [N,H,W,Cout+Cskip]: the UNet up block's norm1 over [hidden | skip].  skip
+ * (16-bit NHWC [N,H,W,Cskip]) may be NULL (Cskip = 0); a group may straddle the two sources.  In the 16-bit modes a
+ * y_conv of Cout <= 512 (Cout % 64 == 0) carries its GroupNorm statistics out of the convolution's epilogue, as in the
+ * engine; otherwise a statistics pass reads it.  Cout, Cskip: multiples of 8. */
+gp_status gp_conv_groupnorm(int dtype, const void* x, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
+                            int Cout, const void* skip, int Cskip, int groups, const float* gamma_host, const float* beta_host,
+                            float eps, int silu, void* y_conv, void* y, void* stream);
 gp_status gp_layernorm(int dtype, const void* x, int64_t tokens, int C, const float* gamma_host,
                        const float* beta_host, float eps, void* y, void* stream);
 /* softmax(q k^T * scale) v per (batch, head); q,k,v,o: 16-bit [B,T,heads*d] */
