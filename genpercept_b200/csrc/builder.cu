@@ -4,8 +4,6 @@
 #include <cmath>
 #include <cstring>
 
-#include <cstdlib>
-
 #include "engine.h"
 #include "fattn.h"
 #include "fattn512.h"
@@ -238,27 +236,9 @@ void Builder::push_igemm(const std::string& name, IgemmParams& p, double flops, 
   ops.back().kind = 1;
 }
 
-// The patch-resident kernel with the GroupNorm transform in its operand path (igemm_patch.cu) takes a convolution when:
-// 3x3 stride 1, ONE normalised source (channels % 64 == 0), at most one raw shortcut source, W % 128 == 0, and either the
-// staged epilogue (Cout % 64 == 0) or an fp32 map as output.  Opt-in (GP_GN_FUSE=1) until it has been timed against the
-// unfused path on H100: it removes the GroupNorm passes over the big maps, but the transform runs inside the consumer
-// warpgroup, between its wgmma batches.
-static bool gn_fusable(const ConvArgs& a, bool split) {
-  const char* on = std::getenv("GP_GN_FUSE");        // read at plan time (tests toggle it)
-  const bool off = on == nullptr || on[0] == '0';
-  if (off || split || a.mode != 0 || a.ks != 3 || a.srcs.size() != 1 || a.sc.size() > 1) return false;
-  const T4& s = a.srcs[0];
-  if ((s.W % 128) || (s.C % 64) || (!a.sc.empty() && (a.sc[0].C % 64))) return false;
-  const int Cout = a.cout_valid > 0 ? a.cout_valid : a.out.C;
-  if (!a.out_f32 && (Cout != a.out.C || (Cout % 64))) return false;
-  if (a.flags & IG_GEGLU) return false;
-  return true;
-}
-
 void Builder::conv(const std::string& name, const ConvArgs& a) {
   GP_REQUIRE(!a.srcs.empty() && a.w != nullptr, name + ": bad conv args");
-  const bool gn_fused = a.gn != nullptr && gn_fusable(a, split_);
-  if (a.gn != nullptr && !gn_fused) {      // materialise GroupNorm(+SiLU)(concat(srcs)), then the plain convolution
+  if (a.gn != nullptr) {      // materialise GroupNorm(+SiLU)(concat(srcs)), then the plain convolution
     int ctot = 0;
     for (auto& s : a.srcs) ctot += s.C;
     T4 tmp = alloc(a.srcs[0].N, a.srcs[0].H, a.srcs[0].W, ctot);
@@ -270,7 +250,6 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
     release(tmp);
     return;
   }
-  if (gn_fused) gn_scale_shift(a.gn_name, a.srcs, *a.gn, a.gn_groups, a.gn_eps);
   const T4& s0 = a.srcs[0];
   const int N = s0.N, H = s0.H, W = s0.W;
   const auto [Ho, Wo] = conv_out_dims(a.mode, H, W);
@@ -302,19 +281,19 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
   const long long work_px = tokens_mode ? ntok : (long long)gw * gh * N * (a.mode == 3 ? 4 : 1);
   int bn_pre = choose_bn(Cout, a.force_bn);
   int mt_pre = (bn_pre <= 64 && work_px >= 256LL * num_sms) ? 2 : 1;
-  if (!a.force_bn && !(a.flags & IG_GEGLU) && !gn_fused) {
+  if (!a.force_bn && !(a.flags & IG_GEGLU)) {
     const double k_elems = flops / (2.0 * N * Ho * Wo * (double)Cout) * (a.mode == 3 ? 4.0 / 9.0 : 1.0);
     tile_shape_for(Cout, k_elems, tokens_mode, N * (a.mode == 3 ? 4 : 1), gw, gh, num_sms, &bn_pre, &mt_pre);
   }
   // the staged (TMA store) epilogue wherever the output allows it; GEGLU and fp32 maps take the direct epilogue
   const bool staged = !a.out_f32 && !(a.flags & IG_GEGLU) && Cout == a.out.C && (Cout % 64) == 0 && (bn_pre % 64) == 0;
-  const bool patch_eligible = gn_fused || (staged && a.mode == 0 && a.ks == 3 && a.srcs.size() == 1 && a.sc.empty() &&
-                                           work_px >= 128LL * num_sms && (W % 128) == 0 && !split_);
-  // The patch-resident kernel takes one image row per tile (two 50 KiB halo patches).  It keeps a planned N tile of 128 with
-  // the staged epilogue, handing the accumulators over in two 64-column halves through a 32 KiB tile, so at least three
-  // 16 KiB weight stages fit with the statistics scratch of any Cout <= 512; every other plan runs at N = 64.
+  const bool patch_eligible = staged && a.mode == 0 && a.ks == 3 && a.srcs.size() == 1 && a.sc.empty() &&
+                              work_px >= 128LL * num_sms && (W % 128) == 0 && !split_;
+  // The patch-resident kernel takes one image row per tile (two 50 KiB halo patches).  It keeps a planned N tile of 128,
+  // handing the accumulators over in two 64-column halves through a 32 KiB tile, so at least three 16 KiB weight stages
+  // fit with the statistics scratch of any Cout <= 512; every other plan runs at N = 64.
   if (patch_eligible) {
-    bn_pre = (bn_pre == 128 && mt_pre == 1 && staged) ? 128 : 64;
+    bn_pre = (bn_pre == 128 && mt_pre == 1) ? 128 : 64;
     mt_pre = 1;
   }
   bool emit_stats = a.want_stats && staged && Cout <= 512 && !split_;
@@ -465,18 +444,6 @@ void Builder::conv(const std::string& name, const ConvArgs& a) {
     p.kc_count = ceil_div(s0.C, 64);
     check_cuda(make_tmap_a(&p.tmPatch, ptr(s0), s0.C, W, H, N, s0.C, (long long)W * s0.C, (long long)H * W * s0.C,
                            p.TW + 2, p.TH + 2, bf16_), name + ": tmap patch");
-    p.tmPatch2 = p.tmPatch;
-    if (!a.sc.empty()) {
-      const T4& x = a.sc[0];
-      p.kc_sc = ceil_div(x.C, 64);
-      check_cuda(make_tmap_a(&p.tmPatch2, ptr(x), x.C, W, H, N, x.C, (long long)W * x.C, (long long)H * W * x.C,
-                             p.TW + 2, p.TH + 2, bf16_), name + ": tmap patch (shortcut)");
-    }
-    if (gn_fused) {
-      p.gn_ss = gn_ss;
-      p.gn_C = s0.C;
-      p.gn_silu = a.gn_silu ? 1 : 0;
-    }
   }
   if (emit_stats) {
     p.stats = reinterpret_cast<float*>(raw_ptr(stats_off));
@@ -661,14 +628,20 @@ void Builder::to_vT(const std::string& name, const T4& l, const PackedW& wv, voi
   push_igemm(name + ".to_vT", p, 2.0 * B * (double)T * C * C, (double)vt_bytes + (double)l.bytes());
 }
 
-// GroupNorm statistics of concat(srcs) over N images of HW pixels -> scale / shift in gn_ss.  Each source's partial sums
-// are either already produced by the conv that wrote it, or computed by a gn_stats pass into a buffer of this op's own
-// (allocated and released here, so both passes make the same arena allocations).  Returns the gn_stats passes +
-// gn_finalize as one launch (empty when measuring); each gn_stats pass adds to `launches` and `bytes`.
-std::function<cudaError_t(cudaStream_t)> Builder::gn_statistics(const std::vector<T4>& srcs, const NormW& nw, int groups,
-                                                                float eps, int N, long long HW, int ctot, int* launches,
-                                                                double* bytes) {
+// GroupNorm(+SiLU) of concat(srcs) into out.  Each source's partial sums are either already produced by the conv that
+// wrote it, or computed by a gn_stats pass into a buffer of this op's own (allocated and released here, so both passes
+// make the same arena allocations).  gn_finalize turns them into a scale / shift per (image, channel) in gn_ss, then one
+// gn_apply pass per source writes its channels of out.
+void Builder::gn(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps,
+                 bool silu, const T4& out) {
+  int ctot = 0;
+  for (auto& s : srcs) ctot += s.C;
+  GP_REQUIRE(ctot == out.C && nw.C == ctot && ctot % groups == 0 && srcs.size() <= 2, name + ": GroupNorm channel mismatch");
+  const int N = out.N;
+  const long long HW = (long long)out.H * out.W;
   const int chunks = gn_chunks(N, HW);
+  int launches = 1;
+  double bytes = (double)out.bytes();
   struct Pass { const void* x; float* partial; int C; };
   std::vector<Pass> passes;
   std::vector<size_t> own;
@@ -682,47 +655,12 @@ std::function<cudaError_t(cudaStream_t)> Builder::gn_statistics(const std::vecto
       float* partial = measuring_ ? nullptr : reinterpret_cast<float*>(raw_ptr(own.back()));
       gs[i] = GnSrc{partial, chunks, srcs[i].C};
       if (!measuring_) passes.push_back(Pass{ptr(srcs[i]), partial, srcs[i].C});
-      ++*launches;
-      *bytes += (double)srcs[i].bytes();
+      ++launches;
+      bytes += (double)srcs[i].bytes();
     }
   }
   for (size_t off : own) arena_.release(off);
-  if (measuring_) return nullptr;
-  float* ss = gn_ss;
-  const bool bf = bf16_, sp = split_;
-  const float* gamma = nw.gamma;
-  const float* beta = nw.beta;
-  return [=](cudaStream_t s) {
-    for (const Pass& q : passes) {
-      cudaError_t e = gn_stats(q.x, N, HW, q.C, q.partial, chunks, q.C, 0, bf, s, sp);
-      if (e != cudaSuccess) return e;
-    }
-    return gn_finalize(gs.data(), (int)gs.size(), gamma, beta, N, ctot, groups, HW, eps, ss, s);
-  };
-}
-
-void Builder::gn_scale_shift(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps) {
-  int ctot = 0;
-  for (auto& s : srcs) ctot += s.C;
-  GP_REQUIRE(nw.C == ctot && ctot % groups == 0 && srcs.size() <= 2 && !srcs.empty(), name + ": GroupNorm channel mismatch");
-  int launches = 1;
-  double bytes = 0;
-  auto stats_fn = gn_statistics(srcs, nw, groups, eps, srcs[0].N, (long long)srcs[0].H * srcs[0].W, ctot, &launches, &bytes);
-  if (!measuring_) push(name, launches, 0, bytes, std::move(stats_fn));
-}
-
-void Builder::gn(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps,
-                 bool silu, const T4& out) {
-  int ctot = 0;
-  for (auto& s : srcs) ctot += s.C;
-  GP_REQUIRE(ctot == out.C && nw.C == ctot && ctot % groups == 0 && srcs.size() <= 2, name + ": GroupNorm channel mismatch");
-  const int N = out.N;
-  const long long HW = (long long)out.H * out.W;
-  int launches = 1;
-  double bytes = (double)out.bytes();
-  auto stats_fn = gn_statistics(srcs, nw, groups, eps, N, HW, ctot, &launches, &bytes);
   if (measuring_) return;
-  // then one apply pass per source
   std::vector<const void*> xs;
   std::vector<int> cs;
   for (auto& s : srcs) {
@@ -734,8 +672,14 @@ void Builder::gn(const std::string& name, const std::vector<T4>& srcs, const Nor
   void* y = ptr(out);
   float* ss = gn_ss;
   const bool bf = bf16_, sp = split_;
+  const float* gamma = nw.gamma;
+  const float* beta = nw.beta;
   push(name, launches, 0, bytes, [=](cudaStream_t s) {
-    cudaError_t e = stats_fn(s);
+    for (const Pass& q : passes) {
+      cudaError_t e = gn_stats(q.x, N, HW, q.C, q.partial, chunks, q.C, 0, bf, s, sp);
+      if (e != cudaSuccess) return e;
+    }
+    cudaError_t e = gn_finalize(gs.data(), (int)gs.size(), gamma, beta, N, ctot, groups, HW, eps, ss, s);
     if (e != cudaSuccess) return e;
     int coff = 0;
     for (size_t i = 0; i < xs.size(); ++i) {
@@ -795,8 +739,7 @@ void Builder::bilinear(const std::string& name, const T4& in, const T4& out) {
   push(name, 1, 0, (double)in.bytes() + out.bytes(), [=](cudaStream_t s) { return bilinear_up2x(xi, yo, t.N, t.H, t.W, t.C, bf, s, sp); });
 }
 
-void Builder::direct(const std::string& name, const T4& in, int cin, const DirectW& w, const T4& out, int flags,
-                     float* out_f32, int up) {
+void Builder::direct(const std::string& name, const T4& in, int cin, const DirectW& w, const T4& out, float* out_f32) {
   GP_REQUIRE(w.Cin == cin, name + ": direct conv channel mismatch");
   if (measuring_) return;
   DirectConvParams p;
@@ -805,10 +748,10 @@ void Builder::direct(const std::string& name, const T4& in, int cin, const Direc
   p.N = in.N; p.H = in.H; p.W = in.W; p.Cin = cin; p.in_cstride = (int)in.ps();
   p.in_lo = split_ ? in.C : 0;
   p.w = w.w; p.bias = w.bias;
-  p.Ho = up ? 2 * in.H : in.H; p.Wo = up ? 2 * in.W : in.W;
+  p.Ho = in.H; p.Wo = in.W;
   p.Cout = w.Cout;
   p.ks = w.ks; p.stride = 1; p.pad = w.ks / 2;
-  p.flags = flags | (up ? DC_UP2X : 0) | (out_f32 ? DC_OUT_F32_NCHW : 0);
+  p.flags = out_f32 ? DC_OUT_F32_NCHW : 0;
   if (out_f32) { p.out = out_f32; p.out_cstride = w.Cout; }
   else { p.out = ptr(out); p.out_cstride = (int)out.ps(); p.out_lo = split_ ? out.C : 0; }
   const bool bf = bf16_;

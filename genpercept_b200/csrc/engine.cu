@@ -113,8 +113,8 @@ struct gp_engine {
     std::vector<int> cs;
     for (auto& x : xs) { cin += x.C; cs.push_back(x.C); }
     const T4& x0 = xs[0];
-    // norm1 -> SiLU -> conv1 and norm2 -> SiLU -> conv2: the normalisation is an attribute of the convolution (fused into
-    // its operand path where the patch-resident kernel applies, materialised by Builder::conv elsewhere)
+    // norm1 -> SiLU -> conv1 and norm2 -> SiLU -> conv2: the normalisation is an attribute of the convolution, which
+    // Builder::conv materialises before it convolves
     T4 h = b.alloc(x0.N, x0.H, x0.W, cout);
     {
       ConvArgs c;
@@ -505,7 +505,7 @@ struct gp_engine {
     T4 h2 = b.alloc(h1.N, h1.H, h1.W, 32);
     { ConvArgs c; c.srcs = {h1}; c.w = &ws.conv_w("dpt.head.head.2", {128}); c.out = h2; c.flags = IG_RELU; b.conv("dpt.head.head.2", c); }
     b.release(h1);
-    b.direct("dpt.head.head.4", h2, 32, ws.direct_w("dpt.head.head.4", 32), h2, 0, out_f32, 0);
+    b.direct("dpt.head.head.4", h2, 32, ws.direct_w("dpt.head.head.4", 32), h2, out_f32);
     const int N = h2.N;
     const long long HW = (long long)h2.H * h2.W;
     *out_h = h2.H; *out_w = h2.W;

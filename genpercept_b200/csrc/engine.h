@@ -121,8 +121,7 @@ struct ConvArgs {
   int force_bn = 0;
   bool want_stats = false;    // let the epilogue emit GroupNorm partial sums of `out` (consumed by Builder::gn)
   // GroupNorm(+SiLU) over concat(srcs) in front of the convolution (norm1 / norm2 / conv_norm_out of the diffusers
-  // blocks).  Where the patch-resident kernel applies, it is fused into the operand path (igemm_patch.cu); elsewhere
-  // Builder::conv materialises the normalised tensor with Builder::gn and convolves that.
+  // blocks).  Builder::conv materialises the normalised tensor with Builder::gn and convolves that.
   const NormW* gn = nullptr;
   std::string gn_name;
   int gn_groups = 32;
@@ -151,14 +150,11 @@ class Builder {
                      int T, int heads, int d, const float* pv_bias, const T4& out, long long qk_lo = 0);
   void gn(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps, bool silu,
           const T4& out);
-  // statistics -> per-(image, channel) scale / shift in gn_ss (the first half of gn(); the apply pass is the caller's)
-  void gn_scale_shift(const std::string& name, const std::vector<T4>& srcs, const NormW& nw, int groups, float eps);
   void ln(const std::string& name, const T4& x, const NormW& nw, float eps, const T4& out);
   void xattn(const std::string& name, const T4& x, const XattnW& w, float eps, const T4& out);
   void relu_op(const std::string& name, const T4& in, const T4& out);
   void bilinear(const std::string& name, const T4& in, const T4& out);
-  void direct(const std::string& name, const T4& in, int cin, const DirectW& w, const T4& out, int flags,
-              float* out_f32, int up);
+  void direct(const std::string& name, const T4& in, int cin, const DirectW& w, const T4& out, float* out_f32);
   void custom(const std::string& name, int launches, double bytes, std::function<cudaError_t(cudaStream_t)> fn);
 
   struct StatsInfo { size_t off; int slots; int C; };
@@ -195,8 +191,6 @@ class Builder {
               long long sN, const std::string& what) const;
   void tmap_b(IgemmParams& p, const void* base, long long lo, long long K, long long rows, long long Z, long long sRow,
               long long sZ, const std::string& what) const;
-  std::function<cudaError_t(cudaStream_t)> gn_statistics(const std::vector<T4>& srcs, const NormW& nw, int groups, float eps,
-                                                         int N, long long HW, int ctot, int* launches, double* bytes);
   bool bf16_, measuring_, split_ = false;
   uint8_t* base_;
   Arena arena_;

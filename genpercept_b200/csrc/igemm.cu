@@ -298,10 +298,9 @@ const char* igemm_finalize(IgemmParams* p) {
   const int fixed = (p->tma_store ? kEpiWarps * 4096 * (p->out_lo ? 2 : 1) : 0) + acc_tile_bytes(*p) + 3072 + stats_bytes;
   const int ring_unit = p->patch ? p->BN * 128 : kABytes * p->MT + p->BN * 128;   // bytes per pipeline stage
   if (p->patch) {
-    if (p->TW != 128 || p->TH != p->MT || p->Z0 != 1 || p->Z1 < 1 || p->nseg[0] != 9 + (p->kc_sc > 0 ? 1 : 0) || p->kc_count < 1 ||
-        p->nkb[0] != 9 * p->kc_count + p->kc_sc || p->npass != 1 || p->gridW % 128 || p->gridH % p->TH)
-      return "patch mode needs TW = 128, TH = MT, full tiles and a single-source 3x3 tap table (+ shortcut chunks)";
-    if (p->gn_ss && p->gn_C != p->kc_count * 64) return "patch mode: GroupNorm channels must equal the source's";
+    if (p->TW != 128 || p->TH != p->MT || p->Z0 != 1 || p->Z1 < 1 || p->nseg[0] != 9 || p->kc_count < 1 ||
+        p->nkb[0] != 9 * p->kc_count || p->npass != 1 || p->gridW % 128 || p->gridH % p->TH || !p->tma_store)
+      return "patch mode needs TW = 128, TH = MT, full tiles, a single-source 3x3 tap table and the staged epilogue";
     p->a_slot_bytes = ((p->TW + 2) * (p->TH + 2) * 128 + 1023) & ~1023;
   }
   const int avail = kMaxSmem - 1024 - fixed - (p->patch ? 2 * p->a_slot_bytes : 0);

@@ -107,15 +107,8 @@ struct IgemmParams {
   // (Cout = 128) layers are bound by exactly that traffic (~42 B/clk/SM of unique data).
   int patch;
   int kc_count;                  // 64-channel K chunks per tap (packed weights are tap-major, kc_count*64 wide per tap)
-  int kc_sc;                     // extra centre-tap-only chunks from tmPatch2 (fused 1x1 shortcut over the raw block input)
   int a_slot_bytes;              // bytes reserved per patch slot (2 slots), multiple of 1024
   CUtensorMap tmPatch;           // (C, W, H, N) view of the source, box (64, TW+2, TH+2, 1)
-  CUtensorMap tmPatch2;          // same box over the shortcut source
-  // GroupNorm(+SiLU) of the patch source applied in shared memory before the MMA reads it (patch mode only):
-  // y = silu(x * scale + shift), (scale, shift) = gn_ss[(image * gn_C + channel) * 2 + {0, 1}] (gn_finalize's output).
-  const float* gn_ss;            // null: the source is used as it is
-  int gn_C;                      // channels of the normalised tensor (= the patch source's)
-  int gn_silu;                   // 1: SiLU after the affine, 0: affine only
 };
 
 cudaError_t igemm_patch_launch(const IgemmParams& p, int grid, cudaStream_t stream);   // igemm_patch.cu

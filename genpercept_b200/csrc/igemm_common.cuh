@@ -14,7 +14,7 @@
 //
 // Registers: the producer warpgroup (warps 8..11, TMA issue only) drops to kProducerRegs per thread at its start and the
 // epilogue and consumer warpgroups rise to kWorkerRegs (128 x 40 + 256 x 232 <= 64 K registers per SM), so the 128
-// accumulators, the transform of the GroupNorm-fused patch kernel and the epilogue's 32-wide vectors fit without spilling.
+// accumulators and the epilogue's 32-wide vectors fit without spilling.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -526,113 +526,11 @@ __global__ void __launch_bounds__(kSmPipeThreads) softmax_rows_pipe_kernel(uint1
 }
 
 // ------------------------------------------------------------------------------ 2-token cross attention
-// y = x + c0 + sigmoid(LN(x).U + u0).M : one warp handles TOK tokens at once so every U / M / c0 vector
-// fetched from L1/L2 is reused TOK times (the single-token version re-read ~2*heads*C*4 bytes per token).
-template <bool BF16, int KV, int TOK>
-__global__ void xattn2_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, long long tokens, int C,
-                              int heads, const float* __restrict__ U, const float* __restrict__ u0,
-                              const float* __restrict__ M, const float* __restrict__ c0, float eps, int lo) {
-  const int lane = threadIdx.x & 31;
-  const long long tok0 = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * TOK;
-  if (tok0 >= tokens) return;
-  const int nvec = C / 8;
-  const int xs = lo ? 2 * C : C;
-  float f[TOK][KV][8];
-  float mean[TOK], rstd[TOK];
-#pragma unroll
-  for (int t = 0; t < TOK; ++t) {
-    const bool tv = tok0 + t < tokens;
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < KV; ++i) {
-      const int v = lane + 32 * i;
-      if (v < nvec && tv) {
-        load8<BF16>(x + (tok0 + t) * xs + v * 8, lo, f[t][i]);
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) f[t][i][e] = 0.f;
-      }
-#pragma unroll
-      for (int e = 0; e < 8; ++e) s += f[t][i][e];
-    }
-    mean[t] = warp_sum(s) / C;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < KV; ++i) {
-      if (lane + 32 * i < nvec) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { const float d = f[t][i][e] - mean[t]; q += d * d; }
-      }
-    }
-    rstd[t] = rsqrtf(warp_sum(q) / C + eps);
-  }
-  float acc[TOK][KV][8];
-#pragma unroll
-  for (int i = 0; i < KV; ++i) {
-    const int v = lane + 32 * i;
-    if (v < nvec) {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(c0 + v * 8));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(c0 + v * 8 + 4));
-#pragma unroll
-      for (int t = 0; t < TOK; ++t) {
-        acc[t][i][0] = f[t][i][0] + a.x; acc[t][i][1] = f[t][i][1] + a.y; acc[t][i][2] = f[t][i][2] + a.z; acc[t][i][3] = f[t][i][3] + a.w;
-        acc[t][i][4] = f[t][i][4] + b.x; acc[t][i][5] = f[t][i][5] + b.y; acc[t][i][6] = f[t][i][6] + b.z; acc[t][i][7] = f[t][i][7] + b.w;
-      }
-    }
-  }
-  for (int h = 0; h < heads; ++h) {
-    float d[TOK];
-#pragma unroll
-    for (int t = 0; t < TOK; ++t) d[t] = 0.f;
-#pragma unroll
-    for (int i = 0; i < KV; ++i) {
-      const int v = lane + 32 * i;
-      if (v < nvec) {
-        const float4 a = __ldg(reinterpret_cast<const float4*>(U + (long long)h * C + v * 8));
-        const float4 b = __ldg(reinterpret_cast<const float4*>(U + (long long)h * C + v * 8 + 4));
-#pragma unroll
-        for (int t = 0; t < TOK; ++t) {
-          const float mt = mean[t];
-          d[t] += (f[t][i][0] - mt) * a.x + (f[t][i][1] - mt) * a.y + (f[t][i][2] - mt) * a.z + (f[t][i][3] - mt) * a.w +
-                  (f[t][i][4] - mt) * b.x + (f[t][i][5] - mt) * b.y + (f[t][i][6] - mt) * b.z + (f[t][i][7] - mt) * b.w;
-        }
-      }
-    }
-    float pr[TOK];
-    const float u0h = __ldg(u0 + h);
-#pragma unroll
-    for (int t = 0; t < TOK; ++t) pr[t] = 1.f / (1.f + __expf(-(warp_sum(d[t]) * rstd[t] + u0h)));
-#pragma unroll
-    for (int i = 0; i < KV; ++i) {
-      const int v = lane + 32 * i;
-      if (v < nvec) {
-        const float4 a = __ldg(reinterpret_cast<const float4*>(M + (long long)h * C + v * 8));
-        const float4 b = __ldg(reinterpret_cast<const float4*>(M + (long long)h * C + v * 8 + 4));
-#pragma unroll
-        for (int t = 0; t < TOK; ++t) {
-          acc[t][i][0] += pr[t] * a.x; acc[t][i][1] += pr[t] * a.y; acc[t][i][2] += pr[t] * a.z; acc[t][i][3] += pr[t] * a.w;
-          acc[t][i][4] += pr[t] * b.x; acc[t][i][5] += pr[t] * b.y; acc[t][i][6] += pr[t] * b.z; acc[t][i][7] += pr[t] * b.w;
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int t = 0; t < TOK; ++t) {
-    if (tok0 + t < tokens) {
-#pragma unroll
-      for (int i = 0; i < KV; ++i) {
-        const int v = lane + 32 * i;
-        if (v < nvec) store8<BF16>(y + (tok0 + t) * xs + v * 8, lo, acc[t][i]);
-      }
-    }
-  }
-}
-
-// Same operator with the folded weights resident in shared memory.  The kernel above re-reads U and M (2 * heads * C
-// floats: 12.8 / 51 / 205 KB at C = 320 / 640 / 1280) through L1 for every warp's tokens — 0.94 GB of L2 traffic per
-// launch at every level.  Here a persistent CTA loads them once,
-// its warps loop over token groups, and the heads are taken five at a time so that the five warp reductions and
-// sigmoids of a batch are independent chains instead of one serial chain per head.
+// y = x + c0 + sigmoid(LN(x).U + u0).M, one warp per TOK tokens so that every U / M / c0 vector read is reused TOK
+// times.  The folded weights live in shared memory: U and M are 2 * heads * C floats (12.8 / 51 / 205 KB at C = 320 /
+// 640 / 1280), and re-reading them through L1 for every warp's tokens costs 0.94 GB of L2 traffic per launch at every
+// level.  A persistent CTA loads them once, its warps loop over token groups, and the heads are taken five at a time so
+// that the five warp reductions and sigmoids of a batch are independent chains instead of one serial chain per head.
 constexpr int kXaHB = 5;
 template <bool BF16, int KV, int TOK>
 __global__ void __launch_bounds__(KV >= 5 ? 512 : 256) xattn2_smem_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, long long tokens,
@@ -1028,63 +926,41 @@ cudaError_t softmax_rows(void* sio, long long rows, int T, int Tp, bool bf16, cu
   return cudaGetLastError();
 }
 
-template <bool BF, int KV, int TOK>
-static cudaError_t xattn2_launch(const void* x, void* y, long long tokens, int C, int heads, const float* U, const float* u0,
-                                 const float* M, const float* c0, float eps, cudaStream_t s, int lo) {
-  const int wpb = 8;
-  const long long per_block = (long long)wpb * TOK;
-  const long long blocks = (tokens + per_block - 1) / per_block;
-  launch(xattn2_kernel<BF, KV, TOK>, (unsigned)blocks, wpb * 32, 0, s, reinterpret_cast<const uint16_t*>(x),
-                                                                    reinterpret_cast<uint16_t*>(y), tokens, C, heads, U, u0, M,
-                                                                    c0, eps, lo);
-  return cudaGetLastError();
-}
-
 cudaError_t xattn2(const void* x, void* y, long long tokens, int C, int heads, const float* U, const float* u0,
                    const float* M, const float* c0, float eps, bool bf16, cudaStream_t s, bool split) {
   const int lo = split ? C : 0;
-  if (C % 8 || C / 8 > 32 * kLnMaxVec) return cudaErrorInvalidValue;
-  const int kv = (C / 8 + 31) / 32;
-  cudaError_t e = cudaSuccess;
   const size_t smem = ((size_t)2 * heads * C + C + heads) * sizeof(float);
-  if (heads % kXaHB == 0 && C % 32 == 0 && smem <= 226 * 1024) {
-    static int sms[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (!sms[dev & 63]) {
-      const int big = 226 * 1024;
-      // the flag is per device, so both storage types get the attribute: an fp16 engine may come first in a process
-      for (const void* f : {(const void*)xattn2_smem_kernel<false, 2, 2>, (const void*)xattn2_smem_kernel<false, 3, 2>,
-                            (const void*)xattn2_smem_kernel<false, 5, 1>, (const void*)xattn2_smem_kernel<true, 2, 2>,
-                            (const void*)xattn2_smem_kernel<true, 3, 2>, (const void*)xattn2_smem_kernel<true, 5, 1>})
-        cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, big);
-      cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
-    }
-    int per_sm = (int)((227 * 1024) / (smem + 1024));
-    if (per_sm > 2) per_sm = 2;                       // 256 threads at <= 128 registers
-    if (per_sm < 1) per_sm = 1;
-    const int tok = kv <= 3 ? 2 : 1;
-    const int threads = kv <= 3 ? 256 : 512;          // C = 1280 leaves room for one CTA per SM: 16 warps instead of 8
-    if (kv > 3) per_sm = 1;
-    long long grid = (tokens + (threads / 32) * tok - 1) / ((threads / 32) * tok);
-    if (grid > (long long)sms[dev & 63] * per_sm) grid = (long long)sms[dev & 63] * per_sm;
-    const uint16_t* xi = reinterpret_cast<const uint16_t*>(x);
-    uint16_t* yo = reinterpret_cast<uint16_t*>(y);
-    if (kv <= 2)
-      GP_DISPATCH_BF16(bf16, (launch(xattn2_smem_kernel<BF, 2, 2>, (unsigned)grid, 256, smem, s, xi, yo, tokens, C, heads, U, u0, M, c0, eps, lo)));
-    else if (kv <= 3)
-      GP_DISPATCH_BF16(bf16, (launch(xattn2_smem_kernel<BF, 3, 2>, (unsigned)grid, 256, smem, s, xi, yo, tokens, C, heads, U, u0, M, c0, eps, lo)));
-    else
-      GP_DISPATCH_BF16(bf16, (launch(xattn2_smem_kernel<BF, 5, 1>, (unsigned)grid, threads, smem, s, xi, yo, tokens, C, heads, U, u0, M, c0, eps, lo)));
-    return cudaGetLastError();
+  if (C % 32 || C / 8 > 32 * kLnMaxVec || heads % kXaHB || smem > 226 * 1024) return cudaErrorInvalidValue;
+  const int kv = (C / 8 + 31) / 32;
+  static int sms[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!sms[dev & 63]) {
+    const int big = 226 * 1024;
+    // the flag is per device, so both storage types get the attribute: an fp16 engine may come first in a process
+    for (const void* f : {(const void*)xattn2_smem_kernel<false, 2, 2>, (const void*)xattn2_smem_kernel<false, 3, 2>,
+                          (const void*)xattn2_smem_kernel<false, 5, 1>, (const void*)xattn2_smem_kernel<true, 2, 2>,
+                          (const void*)xattn2_smem_kernel<true, 3, 2>, (const void*)xattn2_smem_kernel<true, 5, 1>})
+      cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, big);
+    cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
   }
+  int per_sm = (int)((227 * 1024) / (smem + 1024));
+  if (per_sm > 2) per_sm = 2;                       // 256 threads at <= 128 registers
+  if (per_sm < 1) per_sm = 1;
+  const int tok = kv <= 3 ? 2 : 1;
+  const int threads = kv <= 3 ? 256 : 512;          // C = 1280 leaves room for one CTA per SM: 16 warps instead of 8
+  if (kv > 3) per_sm = 1;
+  long long grid = (tokens + (threads / 32) * tok - 1) / ((threads / 32) * tok);
+  if (grid > (long long)sms[dev & 63] * per_sm) grid = (long long)sms[dev & 63] * per_sm;
+  const uint16_t* xi = reinterpret_cast<const uint16_t*>(x);
+  uint16_t* yo = reinterpret_cast<uint16_t*>(y);
   if (kv <= 2)
-    GP_DISPATCH_BF16(bf16, (e = xattn2_launch<BF, 2, 2>(x, y, tokens, C, heads, U, u0, M, c0, eps, s, lo)));
+    GP_DISPATCH_BF16(bf16, (launch(xattn2_smem_kernel<BF, 2, 2>, (unsigned)grid, 256, smem, s, xi, yo, tokens, C, heads, U, u0, M, c0, eps, lo)));
   else if (kv <= 3)
-    GP_DISPATCH_BF16(bf16, (e = xattn2_launch<BF, 3, 1>(x, y, tokens, C, heads, U, u0, M, c0, eps, s, lo)));
+    GP_DISPATCH_BF16(bf16, (launch(xattn2_smem_kernel<BF, 3, 2>, (unsigned)grid, 256, smem, s, xi, yo, tokens, C, heads, U, u0, M, c0, eps, lo)));
   else
-    GP_DISPATCH_BF16(bf16, (e = xattn2_launch<BF, 5, 1>(x, y, tokens, C, heads, U, u0, M, c0, eps, s, lo)));
-  return e;
+    GP_DISPATCH_BF16(bf16, (launch(xattn2_smem_kernel<BF, 5, 1>, (unsigned)grid, threads, smem, s, xi, yo, tokens, C, heads, U, u0, M, c0, eps, lo)));
+  return cudaGetLastError();
 }
 
 cudaError_t relu16(const void* in, void* out, long long n, bool bf16, cudaStream_t s, int split_c) {

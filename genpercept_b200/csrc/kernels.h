@@ -67,6 +67,8 @@ cudaError_t layernorm(const void* x, void* y, long long tokens, int C, const flo
 constexpr int kSoftmaxRowsMaxT = 16384;
 cudaError_t softmax_rows(void* s_inout, long long rows, int T, int Tp, bool bf16, cudaStream_t s, bool split = false);
 // y = x + c0 + sigmoid(LN(x) . U + u0) . M     (SURVEY.md F6; U already carries LN gamma, u0 beta)
+// Needs heads % 5 == 0, C % 32 == 0, C <= 1280 and U, M, c0, u0 within 226 KiB of shared memory (cudaErrorInvalidValue
+// otherwise): the SD-2.1 UNet's 5 / 10 / 20 heads over C = 320 / 640 / 1280.
 cudaError_t xattn2(const void* x, void* y, long long tokens, int C, int heads, const float* U /*[h][C]*/,
                    const float* u0 /*[h]*/, const float* M /*[h][C]*/, const float* c0 /*[C]*/,
                    float eps, bool bf16, cudaStream_t s, bool split = false);

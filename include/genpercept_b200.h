@@ -199,8 +199,7 @@ gp_status gp_groupnorm(int dtype, const void* x, int N, int H, int W, int C, int
                        const float* beta_host, float eps, int silu, void* y, void* stream);
 /* GroupNorm(groups, eps)(+SiLU) -> 3x3 stride-1 convolution (+ optional 1x1 shortcut over a RAW second tensor sc_x
  * [N,H,W,Csc], + optional residual): the norm1/conv1, norm2/conv2 (+conv_shortcut) and conv_norm_out/conv_out pairs of the
- * diffusers ResnetBlock2D / VAE heads.  Where W % 128 == 0 the normalisation runs inside the convolution's operand
- * path (no normalised tensor in HBM), elsewhere as GroupNorm pass + convolution.  y: 16-bit NHWC, or (out_f32 != 0)
+ * diffusers ResnetBlock2D / VAE heads, run as a GroupNorm pass, then the convolution.  y: 16-bit NHWC, or (out_f32 != 0)
  * fp32 NCHW [N,Cout,H,W]. */
 gp_status gp_gn_conv3x3(int dtype, const void* x, int N, int H, int W, int Cin, int groups, const float* gamma_host,
                         const float* beta_host, float eps, int silu, const float* w_host, const float* bias_host, int Cout,

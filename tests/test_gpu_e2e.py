@@ -210,31 +210,6 @@ def test_high_precision_mode_meets_the_stated_tolerance(synth_state, text_embed,
             e.close()
 
 
-def test_groupnorm_fused_graph_matches_the_oracle(synth_state, text_embed, monkeypatch):
-    """GP_GN_FUSE=1: the GroupNorm passes of the W % 128 == 0 VAE layers run inside the consuming convolutions
-    (igemm_patch.cu); same tolerances as the default graph.  256x384: 256- and 384-wide layers take the fused path."""
-    from genpercept_b200.engine import Engine
-    from oracle.pipeline import OraclePipeline
-    monkeypatch.setenv("GP_GN_FUSE", "1")
-    g = torch.Generator().manual_seed(31)
-    rgb = torch.randint(0, 256, (2, 3, 128, 256), generator=g, dtype=torch.uint8)
-    e = Engine(dtype=torch.float16, readout="vae")
-    try:
-        e.load_state("unet", synth_state["unet"]); e.load_state("vae", synth_state["vae"])
-        e.set_text_embed(text_embed)
-        e.finalize()
-        depth = e.infer(rgb.cuda(), out_channels=1).cpu().numpy()
-        normal = e.infer(rgb.cuda(), out_channels=3).cpu().numpy()
-        names = [o["name"] for o in e.profile_ops(out_channels=1)]
-    finally:
-        e.close()
-    assert "vae.decoder.up_blocks.3.resnets.0.norm1" in names                     # scale/shift op only: no gn_apply output tensor
-    p = OraclePipeline(synth_state, text_embed)
-    x = rgb.float() / 255.0 * 2.0 - 1.0
-    assert _report("fused-GN depth", depth, p.single_infer(x, mode="depth").numpy()) < TOL["depth"]
-    assert _report("fused-GN normal", normal, p.single_infer(x, mode="normal").numpy()) < TOL["normal"]
-
-
 def test_mid_size_against_the_oracle(engines, synth_state, text_embed):
     """256x384, batch 2: the largest size the CPU oracle finishes in seconds; exercises the patch-resident conv
     loop (W % 128 == 0), multi-block attention (T = 1536) and the TMA residual path with full tiles."""
