@@ -6,6 +6,7 @@ is missing, construction raises.
 """
 import ctypes
 import os
+import warnings
 from ctypes import POINTER, byref, c_char_p, c_double, c_float, c_int, c_int64, c_size_t, c_void_p
 
 import numpy as np
@@ -94,6 +95,9 @@ def lib():
     L.gp_colorize.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_int,
                               c_void_p]
     L.gp_quantize.argtypes = [c_void_p, c_int, c_size_t, c_int, c_void_p, c_int, c_void_p]
+    L.gp_resize_pil.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p]
+    L.gp_v1_postprocess.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                    c_void_p]
     L.gp_depth_align.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                  c_void_p]
     L.gp_depth_metrics.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_float,
@@ -607,6 +611,55 @@ def quantize(pred, bits=16, to_host=True):
                            _stream_ptr())
     _check_free(st, "gp_quantize")
     return out
+
+
+def resize_pil(img_hwc, out_h, out_w, device=None):
+    """``PIL.Image.Image.resize((out_w, out_h))`` (BICUBIC) of an RGB image, byte for byte, on the GPU (gp_resize_pil).
+    img_hwc: uint8 [H,W,3] numpy array (``np.asarray(pil_image)``) or tensor, host or cuda.  Returns uint8 [3,out_h,out_w]
+    (CHW) on `device` (default: the current cuda device)."""
+    if isinstance(img_hwc, np.ndarray):
+        with warnings.catch_warnings():          # np.asarray of a PIL image is read-only; it is only read here
+            warnings.simplefilter("ignore", UserWarning)
+            x = torch.from_numpy(np.ascontiguousarray(img_hwc))
+    else:
+        x = img_hwc
+    assert x.dtype == torch.uint8 and x.dim() == 3 and x.shape[2] == 3, "an RGB image as uint8 [H,W,3]"
+    x = x.contiguous()
+    H, W = x.shape[:2]
+    out_dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if out_dev.type == "cuda" and out_dev.index is None:
+        out_dev = torch.device("cuda", torch.cuda.current_device())
+    y = torch.empty((3, out_h, out_w), dtype=torch.uint8, device=out_dev)
+    st = lib().gp_resize_pil(c_void_p(x.data_ptr()), _on_host(x), H, W, c_void_p(y.data_ptr()), _on_host(y), out_h, out_w,
+                             _stream_ptr())
+    _check_free(st, "gp_resize_pil")
+    return y
+
+
+V1_TASKS = {"depth": 0, "normal": 1, "seg": 2, "sr": 2}
+
+
+def v1_postprocess(pred, task, size=None):
+    """GenPercept v1's post-processing of the engine's map (gp_v1_postprocess).  pred: cuda fp32 [B,C,h,w] in [0,1];
+    `size` (H, W) or None (no interpolation).  Returns, on the device: depth -> (fp32 [B,H,W] min-max normalised, None);
+    normal -> (fp32 [B,3,H,W] in [-1,1], uint8 [B,H,W,3] norm_to_rgb); seg / sr -> (None, uint8 [B,3,H,W])."""
+    assert pred.is_cuda and pred.dtype == torch.float32 and pred.dim() == 4
+    pred = pred.contiguous()
+    B, C, h, w = pred.shape
+    H, W = (h, w) if size is None else (int(size[0]), int(size[1]))
+    t = V1_TASKS[task]
+    f32 = u8 = None
+    if t == 0:
+        f32 = torch.empty((B, H, W), dtype=torch.float32, device=pred.device)
+    elif t == 1:
+        f32 = torch.empty((B, 3, H, W), dtype=torch.float32, device=pred.device)
+        u8 = torch.empty((B, H, W, 3), dtype=torch.uint8, device=pred.device)
+    else:
+        u8 = torch.empty((B, 3, H, W), dtype=torch.uint8, device=pred.device)
+    st = lib().gp_v1_postprocess(c_void_p(pred.data_ptr()), B, C, h, w, t, H, W, _ptr(f32), _ptr(u8),
+                                 _stream_ptr(pred.device))
+    _check_free(st, "gp_v1_postprocess")
+    return f32, u8
 
 
 def _ptr(t):

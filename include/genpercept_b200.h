@@ -248,6 +248,25 @@ gp_status gp_colorize(const float* pred, int pred_on_host, int B, int H, int W, 
                       const uint8_t* lut768_host, uint8_t* out_hwc, int out_on_host, void* stream);
 /* (pred*255).astype(uint8) / (pred*65535).astype(uint16) of /root/reference/run.py:449-455; bits = 8 or 16. */
 gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, void* out, int out_on_host, void* stream);
+/* replaces: PIL.Image.Image.resize((OW, OH)) with its default filter (BICUBIC, reducing_gap=None) on a mode "RGB" image,
+ * as GenPercept v1's resize_max_res / resize_res call it (GenPercept_v1/genpercept/util/image_util.py).  Byte-identical
+ * to Pillow: the coefficient tables are Pillow's (double, normalised per window, 22-bit fixed point), built on the host
+ * once per (in, out) extent and cached with gp_resize_aa's; the passes are integer only, the horizontal one over just the
+ * rows the vertical one reads, and a pass whose extent is unchanged is skipped.  src: HWC uint8 [H,W,3] (Pillow's
+ * storage order); dst: CHW uint8 [3,OH,OW], the layout gp_infer takes.  Buffers host or device, as gp_resize_aa. */
+gp_status gp_resize_pil(const uint8_t* src_hwc, int src_on_host, int H, int W, uint8_t* dst_chw, int dst_on_host, int OH,
+                        int OW, void* stream);
+/* replaces: the post-processing of GenPercept v1's __call__ (GenPercept_v1/genpercept/pipeline_genpercept.py) on the
+ * engine's map.  pred: fp32 [B,C,h,w] in [0,1] on the device (gp_infer's out); p = 2 pred - 1 is v1's single_infer result.
+ * p is taken to (H, W) by F.interpolate (task 0 / 1: bilinear, align_corners=False, no antialiasing; task 2: the legacy
+ * nearest), skipped when (H, W) == (h, w).  Then, all device buffers:
+ *   task 0 depth (C = 1):  out_f32 [B,H,W] = (x - min) / (max - min) per image, unclamped (a constant map gives NaN);
+ *                          the min / max come from per-block partials reduced in a fixed order
+ *   task 1 normal (C = 3): out_f32 [B,3,H,W] = clip(x, -1, 1); out_u8 [B,H,W,3] = norm_to_rgb of it (float32 arithmetic)
+ *   task 2 seg / sr (C = 3): out_u8 [B,3,H,W] = ((x + 1) / 2 * 255).clip(0, 255).astype(uint8)
+ * Asynchronous on `stream`; shares the pre/post scratch above. */
+gp_status gp_v1_postprocess(const float* pred, int B, int C, int h, int w, int task, int H, int W, float* out_f32,
+                            uint8_t* out_u8, void* stream);
 /* ---- depth evaluation (SURVEY.md §8 f4): the reference's eval.py loop on the device; engine-free ------------------
  * pred, gt: fp32 [B,H,W]; valid: uint8 [B,H,W] (nonzero = valid; NULL = every pixel); all device pointers.  Both
  * calls use the pre/post scratch buffer above, return asynchronously on `stream`, and are bit-identical run to run.
