@@ -739,6 +739,19 @@ void Builder::bilinear(const std::string& name, const T4& in, const T4& out) {
   push(name, 1, 0, (double)in.bytes() + out.bytes(), [=](cudaStream_t s) { return bilinear_up2x(xi, yo, t.N, t.H, t.W, t.C, bf, s, sp); });
 }
 
+void Builder::resize(const std::string& name, const T4& in, const T4& out, bool nearest) {
+  GP_REQUIRE(out.N == in.N && out.C == in.C, name + ": resize shape mismatch");
+  if (measuring_) return;
+  const void* xi = ptr(in);
+  void* yo = ptr(out);
+  const int n = in.N, h = in.H, w = in.W, oh = out.H, ow = out.W, c = in.C;
+  const bool bf = bf16_, sp = split_;
+  const int ch = (int)in.ps();
+  push(name, 1, 0, (double)in.bytes() + (double)out.bytes(), [=](cudaStream_t s) {
+    return nearest ? nearest_resize(xi, yo, n, h, w, oh, ow, ch, s) : bilinear_resize(xi, yo, n, h, w, oh, ow, c, bf, s, sp);
+  });
+}
+
 void Builder::direct(const std::string& name, const T4& in, int cin, const DirectW& w, const T4& out, float* out_f32) {
   GP_REQUIRE(w.Cin == cin, name + ": direct conv channel mismatch");
   if (measuring_) return;

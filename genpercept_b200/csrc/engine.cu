@@ -22,6 +22,81 @@ const int kUnetHeads[4] = {5, 10, 20, 20};
 
 bool is_set(const T4& t) { return t.off >= 0; }
 
+}  // namespace
+
+namespace gp {
+
+T4 resnet_block(Builder& b, WeightStore& ws, const std::string& p, const std::vector<T4>& xs, int cout, float eps, bool temb_on) {
+  int cin = 0;
+  std::vector<int> cs;
+  for (auto& x : xs) { cin += x.C; cs.push_back(x.C); }
+  const T4& x0 = xs[0];
+  // norm1 -> SiLU -> conv1 and norm2 -> SiLU -> conv2: the normalisation is an attribute of the convolution, which
+  // Builder::conv materialises before it convolves
+  T4 h = b.alloc(x0.N, x0.H, x0.W, cout);
+  {
+    ConvArgs c;
+    c.srcs = xs;
+    c.gn = &ws.norm_w(p + ".norm1"); c.gn_name = p + ".norm1"; c.gn_eps = eps;
+    c.w = &ws.resnet_conv1(p, cin, temb_on);
+    c.out = h;
+    c.want_stats = true;     // feeds norm2
+    b.conv(p + ".conv1", c);
+  }
+  T4 out = b.alloc(x0.N, x0.H, x0.W, cout);
+  {
+    ConvArgs c;
+    c.srcs = {h};
+    c.gn = &ws.norm_w(p + ".norm2"); c.gn_name = p + ".norm2"; c.gn_eps = eps;
+    c.out = out;
+    c.want_stats = true;     // resnet outputs feed the next GroupNorm (norm1 / transformer norm / conv_norm_out)
+    if (cin != cout) {
+      c.sc = xs;
+      c.w = &ws.conv_w(p + ".conv2", {cout}, p + ".conv_shortcut", cs);
+    } else {
+      c.w = &ws.conv_w(p + ".conv2", {cout});
+      c.res1 = &xs[0];
+    }
+    b.conv(p + ".conv2", c);
+  }
+  b.release(h);
+  return out;
+}
+
+void cross_attention(Builder& b, WeightStore& ws, const std::string& blk, const T4& x, int heads, float eps, const T4& out) {
+  if (ws.n_tokens == 2) {   // 2-token closed form, fused with its LayerNorm and residual
+    b.xattn(blk + ".attn2", x, ws.xattn_w(blk, x.C, heads), eps, out);
+    return;
+  }
+  // general context length: LN -> [C -> heads*n] GEMM -> per-head softmax -> [heads*n -> C] GEMM + residual
+  const WeightStore::XattnGen xg = ws.xattn_general_w(blk, x.C, heads);
+  T4 l2 = b.alloc(x.N, x.H, x.W, x.C);
+  b.ln(blk + ".norm2", x, ws.norm_w(blk + ".norm2"), eps, l2);
+  T4 sc = b.alloc(x.N, x.H, x.W, xg.Kp);
+  { ConvArgs c; c.srcs = {l2}; c.ks = 1; c.w = xg.A; c.out = sc; b.conv(blk + ".attn2.scores", c); }
+  b.release(l2);
+  if (!b.measuring()) {
+    void* sp = b.ptr(sc);
+    const long long rows = x.pixels();
+    const int kp = xg.Kp, nh = heads, nt = ws.n_tokens;
+    const bool bf = b.bf16(), spl = b.split();
+    b.custom(blk + ".attn2.softmax", 1, 2.0 * rows * kp * 2,
+             [=](cudaStream_t s) { return softmax_groups(sp, rows, kp, nh, nt, bf, s, spl); });
+  }
+  { ConvArgs c; c.srcs = {sc}; c.ks = 1; c.w = xg.B; c.out = out; c.res1 = &x; b.conv(blk + ".attn2.out", c); }
+  b.release(sc);
+}
+
+void geglu_projection(Builder& b, WeightStore& ws, const std::string& blk, const T4& x, const T4& out) {
+  ConvArgs c; c.srcs = {x}; c.ks = 1; c.w = &ws.geglu_w(blk, x.C); c.out = out; c.cout_valid = 8 * x.C;
+  c.flags = IG_GEGLU; c.force_bn = 128;
+  b.conv(blk + ".ff.proj_geglu", c);
+}
+
+}  // namespace gp
+
+namespace {
+
 struct Plan {
   int B = 0, H = 0, W = 0;
   uint8_t* arena = nullptr;
@@ -108,43 +183,6 @@ struct gp_engine {
     b.conv(key, c);
   }
 
-  T4 resnet(Builder& b, const std::string& p, const std::vector<T4>& xs, int cout, float eps, bool temb_on) {
-    int cin = 0;
-    std::vector<int> cs;
-    for (auto& x : xs) { cin += x.C; cs.push_back(x.C); }
-    const T4& x0 = xs[0];
-    // norm1 -> SiLU -> conv1 and norm2 -> SiLU -> conv2: the normalisation is an attribute of the convolution, which
-    // Builder::conv materialises before it convolves
-    T4 h = b.alloc(x0.N, x0.H, x0.W, cout);
-    {
-      ConvArgs c;
-      c.srcs = xs;
-      c.gn = &ws.norm_w(p + ".norm1"); c.gn_name = p + ".norm1"; c.gn_eps = eps;
-      c.w = &ws.resnet_conv1(p, cin, temb_on);
-      c.out = h;
-      c.want_stats = true;     // feeds norm2
-      b.conv(p + ".conv1", c);
-    }
-    T4 out = b.alloc(x0.N, x0.H, x0.W, cout);
-    {
-      ConvArgs c;
-      c.srcs = {h};
-      c.gn = &ws.norm_w(p + ".norm2"); c.gn_name = p + ".norm2"; c.gn_eps = eps;
-      c.out = out;
-      c.want_stats = true;     // resnet outputs feed the next GroupNorm (norm1 / transformer norm / conv_norm_out)
-      if (cin != cout) {
-        c.sc = xs;
-        c.w = &ws.conv_w(p + ".conv2", {cout}, p + ".conv_shortcut", cs);
-      } else {
-        c.w = &ws.conv_w(p + ".conv2", {cout});
-        c.res1 = &xs[0];
-      }
-      b.conv(p + ".conv2", c);
-    }
-    b.release(h);
-    return out;
-  }
-
   T4 transformer(Builder& b, const std::string& p, const T4& x, int heads) {
     const int C = x.C;
     const std::string blk = p + ".transformer_blocks.0";
@@ -163,38 +201,15 @@ struct gp_engine {
     { ConvArgs c; c.srcs = {o}; c.ks = 1; c.w = &ws.lin_w(blk + ".attn1.to_out.0"); c.out = t1; c.res1 = &t; b.conv(blk + ".attn1.to_out", c); }
     b.release(o);
     b.release(t);
-    // cross attention (2-token closed form, fused with its LayerNorm and residual)
+    // cross attention
     T4 t2 = b.alloc(x.N, x.H, x.W, C);
-    if (ws.n_tokens == 2) {
-      b.xattn(blk + ".attn2", t1, ws.xattn_w(blk, C, heads), 1e-5f, t2);
-    } else {   // general context length: LN -> [C -> heads*n] GEMM -> per-head softmax -> [heads*n -> C] GEMM + residual
-      const WeightStore::XattnGen xg = ws.xattn_general_w(blk, C, heads);
-      T4 l2 = b.alloc(x.N, x.H, x.W, C);
-      b.ln(blk + ".norm2", t1, ws.norm_w(blk + ".norm2"), 1e-5f, l2);
-      T4 sc = b.alloc(x.N, x.H, x.W, xg.Kp);
-      { ConvArgs c; c.srcs = {l2}; c.ks = 1; c.w = xg.A; c.out = sc; b.conv(blk + ".attn2.scores", c); }
-      b.release(l2);
-      if (!b.measuring()) {
-        void* sp = b.ptr(sc);
-        const long long rows = (long long)x.N * x.H * x.W;
-        const int kp = xg.Kp, nh = heads, nt = ws.n_tokens;
-        const bool bf = b.bf16(), spl = b.split();
-        b.custom(blk + ".attn2.softmax", 1, 2.0 * rows * kp * 2,
-                 [=](cudaStream_t s) { return softmax_groups(sp, rows, kp, nh, nt, bf, s, spl); });
-      }
-      { ConvArgs c; c.srcs = {sc}; c.ks = 1; c.w = xg.B; c.out = t2; c.res1 = &t1; b.conv(blk + ".attn2.out", c); }
-      b.release(sc);
-    }
+    cross_attention(b, ws, blk, t1, heads, 1e-5f, t2);
     b.release(t1);
     // feed-forward (GEGLU)
     T4 l3 = b.alloc(x.N, x.H, x.W, C);
     b.ln(blk + ".norm3", t2, ws.norm_w(blk + ".norm3"), 1e-5f, l3);
     T4 gg = b.alloc(x.N, x.H, x.W, 4 * C);
-    {
-      ConvArgs c; c.srcs = {l3}; c.ks = 1; c.w = &ws.geglu_w(blk, C); c.out = gg; c.cout_valid = 8 * C;
-      c.flags = IG_GEGLU; c.force_bn = 128;
-      b.conv(blk + ".ff.proj_geglu", c);
-    }
+    geglu_projection(b, ws, blk, l3, gg);
     b.release(l3);
     T4 t3 = b.alloc(x.N, x.H, x.W, C);
     { ConvArgs c; c.srcs = {gg}; c.ks = 1; c.w = &ws.lin_w(blk + ".ff.net.2"); c.out = t3; c.res1 = &t2; b.conv(blk + ".ff.out", c); }
@@ -207,7 +222,7 @@ struct gp_engine {
   }
 
   T4 vae_mid(Builder& b, const std::string& p, T4 x) {
-    T4 r0 = resnet(b, p + ".resnets.0", {x}, 512, 1e-6f, false);
+    T4 r0 = resnet_block(b, ws,p + ".resnets.0", {x}, 512, 1e-6f, false);
     b.release(x);
     const std::string a = p + ".attentions.0";
     T4 n = b.alloc(r0.N, r0.H, r0.W, 512);
@@ -219,7 +234,7 @@ struct gp_engine {
     { ConvArgs c; c.srcs = {o}; c.ks = 1; c.w = &ws.lin_w(a + ".to_out.0"); c.out = y; c.res1 = &r0; c.want_stats = true; b.conv(a + ".to_out", c); }
     b.release(o);
     b.release(r0);
-    T4 r1 = resnet(b, p + ".resnets.1", {y}, 512, 1e-6f, false);
+    T4 r1 = resnet_block(b, ws,p + ".resnets.1", {y}, 512, 1e-6f, false);
     b.release(y);
     return r1;
   }
@@ -240,7 +255,7 @@ struct gp_engine {
     const int ch[5] = {128, 128, 256, 512, 512};
     for (int i = 0; i < 4; ++i) {
       for (int j = 0; j < 2; ++j) {
-        T4 y = resnet(b, e + ".down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), {x}, ch[i + 1], 1e-6f, false);
+        T4 y = resnet_block(b, ws,e + ".down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), {x}, ch[i + 1], 1e-6f, false);
         b.release(x);
         x = y;
       }
@@ -281,7 +296,7 @@ struct gp_engine {
       const int cout = kUnetOut[i];
       for (int j = 0; j < 2; ++j) {
         const std::string rp = u + ".down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j);
-        T4 y = resnet(b, rp, {x}, cout, 1e-5f, true);
+        T4 y = resnet_block(b, ws,rp, {x}, cout, 1e-5f, true);
         if (i < 3) {
           T4 y2 = transformer(b, u + ".down_blocks." + std::to_string(i) + ".attentions." + std::to_string(j), y, kUnetHeads[i]);
           b.release(y);
@@ -301,10 +316,10 @@ struct gp_engine {
       }
     }
     // mid block; x (the last skip) stays alive for the up path
-    T4 m0 = resnet(b, u + ".mid_block.resnets.0", {x}, 1280, 1e-5f, true);
+    T4 m0 = resnet_block(b, ws,u + ".mid_block.resnets.0", {x}, 1280, 1e-5f, true);
     T4 m1 = transformer(b, u + ".mid_block.attentions.0", m0, 20);
     b.release(m0);
-    T4 cur = resnet(b, u + ".mid_block.resnets.1", {m1}, 1280, 1e-5f, true);
+    T4 cur = resnet_block(b, ws,u + ".mid_block.resnets.1", {m1}, 1280, 1e-5f, true);
     b.release(m1);
     const int up_out[4] = {1280, 1280, 640, 320};
     const bool up_attn[4] = {false, true, true, true};
@@ -314,7 +329,7 @@ struct gp_engine {
         T4 skip = skips.back();
         skips.pop_back();
         const std::string rp = u + ".up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j);
-        T4 y = resnet(b, rp, {cur, skip}, up_out[i], 1e-5f, true);
+        T4 y = resnet_block(b, ws,rp, {cur, skip}, up_out[i], 1e-5f, true);
         b.release(cur);
         b.release(skip);
         if (up_attn[i]) {
@@ -342,13 +357,7 @@ struct gp_engine {
           GP_REQUIRE(nxt.H <= 2 * cur.H && nxt.H >= 2 * cur.H - 1 && nxt.W <= 2 * cur.W && nxt.W >= 2 * cur.W - 1,
                      "unexpected skip size in the UNet up path");
           T4 up = b.alloc(cur.N, nxt.H, nxt.W, cur.C);
-          if (!b.measuring()) {
-            const void* src = b.ptr(cur);
-            void* dst = b.ptr(up);
-            const int n = cur.N, h = cur.H, w = cur.W, oh = nxt.H, ow = nxt.W, ch = (int)cur.ps();   // both planes move together
-            b.custom(k + ".nearest", 1, (double)cur.bytes() + (double)up.bytes(),
-                     [=](cudaStream_t s) { return nearest_resize(src, dst, n, h, w, oh, ow, ch, s); });
-          }
+          b.resize(k + ".nearest", cur, up, true);
           b.release(cur);
           T4 y = b.alloc(up.N, up.H, up.W, up.C);
           ConvArgs c; c.srcs = {up}; c.mode = 0; c.w = &plain; c.out = y; c.want_stats = true;
@@ -399,7 +408,7 @@ struct gp_engine {
     const int oc[4] = {512, 512, 256, 128};
     for (int i = 0; i < 4; ++i) {
       for (int j = 0; j < 3; ++j) {
-        T4 y = resnet(b, d + ".up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), {x}, oc[i], 1e-6f, false);
+        T4 y = resnet_block(b, ws,d + ".up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), {x}, oc[i], 1e-6f, false);
         b.release(x);
         x = y;
       }
@@ -470,14 +479,7 @@ struct gp_engine {
         const bool rs = x.H != f.H || x.W != f.W;
         if (rs) {
           fr = b.alloc(x.N, x.H, x.W, 256);
-          if (!b.measuring()) {
-            const void* src = b.ptr(f);
-            void* dst = b.ptr(fr);
-            const int n = f.N, h = f.H, w = f.W, oh = x.H, ow = x.W;
-            const bool bf = b.bf16(), spl = b.split();
-            b.custom(lp + ".resize_skip", 1, (double)f.bytes() + (double)fr.bytes(),
-                     [=](cudaStream_t st) { return bilinear_resize(src, dst, n, h, w, oh, ow, 256, bf, st, spl); });
-          }
+          b.resize(lp + ".resize_skip", f, fr, false);
         }
         T4 s = dpt_rcu(b, lp + ".residual_layer1", fr, &x);   // x + (f + conv2(...))
         if (rs) b.release(fr);

@@ -154,6 +154,9 @@ class Builder {
   void xattn(const std::string& name, const T4& x, const XattnW& w, float eps, const T4& out);
   void relu_op(const std::string& name, const T4& in, const T4& out);
   void bilinear(const std::string& name, const T4& in, const T4& out);
+  // F.interpolate(size=(out.H, out.W)) of `in`: nearest (a gather of whole pixels, both planes of the (hi, lo) layout at
+  // once) or bilinear with align_corners=False
+  void resize(const std::string& name, const T4& in, const T4& out, bool nearest);
   void direct(const std::string& name, const T4& in, int cin, const DirectW& w, const T4& out, float* out_f32);
   void custom(const std::string& name, int launches, double bytes, std::function<cudaError_t(cudaStream_t)> fn);
 
@@ -277,6 +280,17 @@ class WeightStore {
   std::vector<float> te_w1, te_b1, te_w2, te_b2;
   std::map<int, std::vector<std::vector<float>>> temb_cache;   // timestep -> folded bias per layer
 };
+
+// engine.cu: pieces of the SD-2.1 UNet emitted on `b` over the weights `ws` holds under a checkpoint prefix.  The engine's
+// graph and the per-kernel entry points (kernel_entry.cu) emit the same ops through them.
+// ResnetBlock2D over concat(xs) (one or two sources) with 32 groups; temb_on folds the time embedding into conv1's bias.
+// Returns a new arena tensor of `cout` channels whose GroupNorm statistics come with it where the epilogue makes them.
+T4 resnet_block(Builder& b, WeightStore& ws, const std::string& p, const std::vector<T4>& xs, int cout, float eps, bool temb_on);
+// out = x + attn2(norm2(x), context) of transformer block `blk`: the 2-token closed form when ws.n_tokens == 2, else LN ->
+// scores GEMM -> per-head softmax -> output GEMM with the residual.
+void cross_attention(Builder& b, WeightStore& ws, const std::string& blk, const T4& x, int heads, float eps, const T4& out);
+// out [.., 4C] = GEGLU(ff.net.0.proj(x)) of transformer block `blk` (x [.., C], the projection's GEGLU epilogue)
+void geglu_projection(Builder& b, WeightStore& ws, const std::string& blk, const T4& x, const T4& out);
 
 // arena.cu: the per-device activation arena shared by the plans of engines with gp_set_shared_arena on.  join / leave
 // count the engines that share it (the last leave unmaps everything and frees the reservation); add maps enough for a

@@ -319,6 +319,107 @@ gp_status gp_bilinear_up2x(int dtype, const void* x, int N, int H, int W, int C,
   });
 }
 
+gp_status gp_geglu(int dtype, const void* x, int64_t tokens, int C, const float* w_host, const float* b_host, void* y,
+                   void* stream) {
+  return guarded_free([&]() {
+    GP_REQUIRE(x && y && w_host && b_host && tokens >= 1 && tokens < (1LL << 31) && C >= 8 && C % 8 == 0,
+               "gp_geglu: bad arguments (C % 8 == 0)");
+    const bool pair = storage_layout(dtype, true, "gp_geglu");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    WeightStore ws(dtype == GP_BF16, pair);
+    ws.put("t.ff.net.0.proj.weight", {8LL * C, C}, w_host);
+    ws.put("t.ff.net.0.proj.bias", {8LL * C}, b_host);
+    build_and_run(ws, s, [&](Builder& b) {
+      geglu_projection(b, ws, "t", b.external(x, 1, 1, (int)tokens, C), b.external(y, 1, 1, (int)tokens, 4 * C));
+    });
+  });
+}
+
+gp_status gp_cross_attention(int dtype, const void* x, int64_t tokens, int C, int heads, const float* ctx_host, int n, int E,
+                             const float* to_q, const float* to_k, const float* to_v, const float* to_out_w,
+                             const float* to_out_b, const float* norm_g, const float* norm_b, float eps, void* y,
+                             void* stream) {
+  return guarded_free([&]() {
+    GP_REQUIRE(x && y && ctx_host && to_q && to_k && to_v && to_out_w && to_out_b && norm_g && norm_b && tokens >= 1 &&
+                   tokens < (1LL << 31) && heads >= 1 && C % heads == 0 && C % 8 == 0 && n >= 1 && E >= 1,
+               "gp_cross_attention: bad arguments (C % 8 == 0, C % heads == 0)");
+    const bool pair = storage_layout(dtype, true, "gp_cross_attention");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    WeightStore ws(dtype == GP_BF16, pair);
+    ws.text_embed.assign(ctx_host, ctx_host + (size_t)n * E);
+    ws.n_tokens = n;
+    ws.put("t.attn2.to_q.weight", {C, C}, to_q);
+    ws.put("t.attn2.to_k.weight", {C, E}, to_k);
+    ws.put("t.attn2.to_v.weight", {C, E}, to_v);
+    ws.put("t.attn2.to_out.0.weight", {C, C}, to_out_w);
+    ws.put("t.attn2.to_out.0.bias", {C}, to_out_b);
+    ws.put("t.norm2.weight", {C}, norm_g);
+    ws.put("t.norm2.bias", {C}, norm_b);
+    build_and_run(ws, s, [&](Builder& b) {
+      const int T = (int)tokens;
+      cross_attention(b, ws, "t", b.external(x, 1, 1, T, C), heads, eps, b.external(y, 1, 1, T, C));
+    });
+  });
+}
+
+gp_status gp_resnet(int dtype, const void* x, int Cx, const void* skip, int Cskip, int N, int H, int W, int Cout, float eps,
+                    const float* norm1_g, const float* norm1_b, const float* conv1_w, const float* conv1_b,
+                    const float* norm2_g, const float* norm2_b, const float* conv2_w, const float* conv2_b,
+                    const float* shortcut_w, const float* shortcut_b, void* y, void* stream) {
+  return guarded_free([&]() {
+    const int Cin = Cx + Cskip;
+    GP_REQUIRE(x && y && norm1_g && norm1_b && conv1_w && conv1_b && norm2_g && norm2_b && conv2_w && conv2_b && N >= 1 &&
+                   H >= 1 && W >= 1 && Cx >= 8 && Cx % 8 == 0 && Cskip % 8 == 0 && (skip ? Cskip > 0 : Cskip == 0) &&
+                   Cin % 32 == 0 && Cout >= 32 && Cout % 32 == 0,
+               "gp_resnet: bad arguments (channels: multiples of 8, Cx + Cskip and Cout of 32)");
+    GP_REQUIRE((shortcut_w && shortcut_b) == (Cin != Cout) && (shortcut_w != nullptr) == (shortcut_b != nullptr),
+               "gp_resnet: the shortcut weights are required exactly when Cx + Cskip != Cout");
+    const bool pair = storage_layout(dtype, true, "gp_resnet");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    WeightStore ws(dtype == GP_BF16, pair);
+    ws.put("t.norm1.weight", {Cin}, norm1_g);
+    ws.put("t.norm1.bias", {Cin}, norm1_b);
+    ws.put("t.conv1.weight", {Cout, Cin, 3, 3}, conv1_w);
+    ws.put("t.conv1.bias", {Cout}, conv1_b);
+    ws.put("t.norm2.weight", {Cout}, norm2_g);
+    ws.put("t.norm2.bias", {Cout}, norm2_b);
+    ws.put("t.conv2.weight", {Cout, Cout, 3, 3}, conv2_w);
+    ws.put("t.conv2.bias", {Cout}, conv2_b);
+    if (shortcut_w) {
+      ws.put("t.conv_shortcut.weight", {Cout, Cin, 1, 1}, shortcut_w);
+      ws.put("t.conv_shortcut.bias", {Cout}, shortcut_b);
+    }
+    float* ss = ws.upload(std::vector<float>((size_t)N * std::max(Cin, Cout) * 2, 0.f));
+    build_and_run(ws, s, [&](Builder& b) {
+      b.gn_ss = ss;
+      std::vector<T4> xs = {b.external(x, N, H, W, Cx)};
+      if (skip) xs.push_back(b.external(skip, N, H, W, Cskip));
+      const T4 out = resnet_block(b, ws, "t", xs, Cout, eps, false);
+      // the block writes a tensor of the arena; the caller's y takes a copy
+      if (!b.measuring()) {
+        const void* src = b.ptr(out);
+        const size_t nb = out.bytes();
+        b.custom("gp_resnet.out", 1, 2.0 * nb,
+                 [=](cudaStream_t st) { return cudaMemcpyAsync(y, src, nb, cudaMemcpyDeviceToDevice, st); });
+      }
+      b.release(out);
+    });
+  });
+}
+
+gp_status gp_resize(int dtype, const void* x, int N, int H, int W, int C, int OH, int OW, int mode, void* y, void* stream) {
+  return guarded_free([&]() {
+    GP_REQUIRE(x && y && N >= 1 && H >= 1 && W >= 1 && OH >= 1 && OW >= 1 && C >= 8 && C % 8 == 0 && (mode == 0 || mode == 1),
+               "gp_resize: bad arguments (C % 8 == 0, mode 0 nearest or 1 bilinear)");
+    const bool pair = storage_layout(dtype, true, "gp_resize");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    WeightStore ws(dtype == GP_BF16, pair);
+    build_and_run(ws, s, [&](Builder& b) {
+      b.resize("gp_resize", b.external(x, N, H, W, C), b.external(y, N, OH, OW, C), mode == 0);
+    });
+  });
+}
+
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters, double* usec,
                         double* flops) {
   return guarded_free([&]() {

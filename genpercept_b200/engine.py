@@ -85,6 +85,12 @@ def lib():
     L.gp_attention.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                c_void_p]
     L.gp_bilinear_up2x.argtypes = [c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    L.gp_geglu.argtypes = [c_int, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.gp_cross_attention.argtypes = [c_int, c_void_p, c_int64, c_int, c_int, c_void_p, c_int, c_int] + [c_void_p] * 7 + \
+        [c_float, c_void_p, c_void_p]
+    L.gp_resnet.argtypes = [c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float] + [c_void_p] * 10 + \
+        [c_void_p, c_void_p]
+    L.gp_resize.argtypes = [c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
     L.gp_bench_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_double),
                                 POINTER(c_double)]
     L.gp_bench_attention.argtypes = [c_int, c_int, c_int, c_int, c_int, POINTER(c_double), POINTER(c_double)]
@@ -557,6 +563,67 @@ def bilinear_up2x(x_nhwc):
     y = _out((N, 2 * H, 2 * W, C), dt, x_nhwc.device)
     st = lib().gp_bilinear_up2x(dt, c_void_p(x.data_ptr()), N, H, W, C, c_void_p(y.data_ptr()), _stream_ptr())
     _check_free(st, "gp_bilinear_up2x")
+    return _result(y, dt)
+
+
+def _host_f32(t):
+    """A weight (or None) as the per-kernel entry points take it: contiguous fp32 on the host."""
+    return None if t is None else t.detach().float().cpu().contiguous()
+
+
+def geglu(x, w, b):
+    """GEGLU(x @ w^T + b) through gp_geglu: x cuda [tokens, C] (f16/bf16, or fp32: the pair layout, float64 result); w [8C, C]
+    and b [8C] as ff.net.0.proj stores them.  Returns [tokens, 4C]."""
+    dt = _layout(x)
+    T, C = x.shape
+    xa = _arg(x, dt)
+    y = _out((T, 4 * C), dt, x.device)
+    w_, b_ = _host_f32(w), _host_f32(b)
+    _check_free(lib().gp_geglu(dt, _ptr(xa), T, C, _ptr(w_), _ptr(b_), _ptr(y), _stream_ptr(x.device)), "gp_geglu")
+    return _result(y, dt)
+
+
+def cross_attention(x, ctx, heads, to_q, to_k, to_v, to_out_w, to_out_b, norm_g, norm_b, eps=1e-5):
+    """x + attn2(LayerNorm(x), ctx) through gp_cross_attention: x cuda [tokens, C] (f16/bf16, or fp32: the pair layout,
+    float64 result); ctx [n, E] and the weights in the checkpoint's layout.  n = 2 runs the closed form."""
+    dt = _layout(x)
+    T, C = x.shape
+    n, Ed = ctx.shape
+    xa = _arg(x, dt)
+    y = _out((T, C), dt, x.device)
+    hs = [_host_f32(t) for t in (ctx, to_q, to_k, to_v, to_out_w, to_out_b, norm_g, norm_b)]
+    st = lib().gp_cross_attention(dt, _ptr(xa), T, C, heads, _ptr(hs[0]), n, Ed, *[_ptr(t) for t in hs[1:]], eps, _ptr(y),
+                                  _stream_ptr(x.device))
+    _check_free(st, "gp_cross_attention")
+    return _result(y, dt)
+
+
+def resnet(x_nhwc, skip, cout, eps, norm1, conv1, norm2, conv2, shortcut=None):
+    """ResnetBlock2D (32 groups, no time embedding) over concat(x, skip) through gp_resnet: x / skip NHWC cuda (f16/bf16,
+    or fp32: the pair layout, float64 result); norm1 / norm2 = (gamma, beta), conv1 / conv2 / shortcut = (weight, bias).
+    Returns NHWC [N, H, W, cout]."""
+    dt = _layout(x_nhwc)
+    N, H, W, Cx = x_nhwc.shape
+    Cskip = 0 if skip is None else skip.shape[-1]
+    xa, sk = _arg(x_nhwc, dt), _arg(skip, dt)
+    y = _out((N, H, W, cout), dt, x_nhwc.device)
+    ws = [_host_f32(t) for pair in (norm1, conv1, norm2, conv2, shortcut or (None, None)) for t in pair]
+    st = lib().gp_resnet(dt, _ptr(xa), Cx, _ptr(sk), Cskip, N, H, W, cout, eps, *[_ptr(t) for t in ws], _ptr(y),
+                         _stream_ptr(x_nhwc.device))
+    _check_free(st, "gp_resnet")
+    return _result(y, dt)
+
+
+def resize(x_nhwc, out_h, out_w, mode):
+    """F.interpolate(size=(out_h, out_w)) of NHWC x through gp_resize: mode "nearest", or "bilinear" (align_corners=False).
+    f16/bf16, or fp32: the pair layout, float64 result."""
+    dt = _layout(x_nhwc)
+    N, H, W, C = x_nhwc.shape
+    xa = _arg(x_nhwc, dt)
+    y = _out((N, out_h, out_w, C), dt, x_nhwc.device)
+    st = lib().gp_resize(dt, _ptr(xa), N, H, W, C, out_h, out_w, {"nearest": 0, "bilinear": 1}[mode], _ptr(y),
+                         _stream_ptr(x_nhwc.device))
+    _check_free(st, "gp_resize")
     return _result(y, dt)
 
 

@@ -184,8 +184,8 @@ gp_status gp_op_info(gp_engine* e, int64_t i, char* name_buf, size_t name_cap, d
                      double* bytes, int* kind, double* flops_exec);
 
 /* ---- per-kernel entry points (parity tests, micro-benchmarks); all pointers are device ----
- * dtype: GP_F16 or GP_BF16; gp_conv2d, gp_groupnorm, gp_gn_conv3x3, gp_conv_groupnorm, gp_layernorm and
- * gp_bilinear_up2x also take GP_F16_PAIR, in which every 16-bit tensor (inputs, residual, skip, shortcut, outputs) has
+ * dtype: GP_F16 or GP_BF16; gp_conv2d, gp_groupnorm, gp_gn_conv3x3, gp_conv_groupnorm, gp_layernorm,
+ * gp_bilinear_up2x and the UNet block ops (gp_geglu .. gp_resize) also take GP_F16_PAIR, in which every 16-bit tensor (inputs, residual, skip, shortcut, outputs) has
  * the [hi C | lo C] layout and the contractions run the high-precision mode's three passes (hi*hi + lo*hi + hi*lo). */
 /* 3x3 / 1x1 convolution through the wgmma implicit-GEMM kernels.  x: 16-bit NHWC [N,H,W,Cin];
  * w: fp32 [Cout,Cin,ks,ks] (host); mode: 0 stride-1 pad ks/2, 1 stride-2 pad (1,1,1,1),
@@ -231,6 +231,31 @@ gp_status gp_attention_high(const void* qk, const void* v, int B, int T, int hea
 gp_status gp_ensemble_reduce(const float* pred_dev, int B, int H, int W, const float* scale_host, const float* shift_host,
                              int median, int normalise, float* out_dev, void* stream);
 gp_status gp_bilinear_up2x(int dtype, const void* x, int N, int H, int W, int C, void* y, void* stream);
+/* The UNet transformer's and up blocks' ops through the engine's own emission (the same ops, weights folding and packing
+ * as a plan), each on caller buffers, synchronised.  dtype: GP_F16, GP_BF16 or GP_F16_PAIR; weights fp32 on the host, in
+ * the checkpoint's layout.
+ * gp_geglu: y [tokens,4C] = GEGLU(x [tokens,C] @ w^T + b), w [8C,C] and b [8C] as ff.net.0.proj stores them (values in rows
+ * 0..4C-1, gates in 4C..8C-1; GELU with erf).  C % 8 == 0. */
+gp_status gp_geglu(int dtype, const void* x, int64_t tokens, int C, const float* w_host, const float* b_host, void* y,
+                   void* stream);
+/* y [tokens,C] = x + attn2(LayerNorm(x; norm_g, norm_b, eps), ctx) with `heads` heads: to_q [C,C], to_k / to_v [C,E],
+ * to_out [C,C] + [C], ctx [n,E] (host).  n = 2 takes the closed-form 2-token kernel (heads % 5 == 0, C <= 1280), any other n
+ * the general path (LayerNorm, scores GEMM, per-head softmax, output GEMM).  C % 8 == 0, C % heads == 0. */
+gp_status gp_cross_attention(int dtype, const void* x, int64_t tokens, int C, int heads, const float* ctx_host, int n, int E,
+                             const float* to_q, const float* to_k, const float* to_v, const float* to_out_w,
+                             const float* to_out_b, const float* norm_g, const float* norm_b, float eps, void* y,
+                             void* stream);
+/* ResnetBlock2D (32 groups, SiLU, no time embedding) over concat(x [N,H,W,Cx], skip [N,H,W,Cskip]) -> y [N,H,W,Cout]:
+ * norm1 [Cin], conv1 [Cout,Cin,3,3] + [Cout], norm2 [Cout], conv2 [Cout,Cout,3,3] + [Cout], and the 1x1 conv_shortcut
+ * [Cout,Cin,1,1] + [Cout], given exactly when Cin = Cx + Cskip != Cout (else the residual is x).  skip may be NULL
+ * (Cskip = 0).  Channels: multiples of 8, Cin and Cout of 32. */
+gp_status gp_resnet(int dtype, const void* x, int Cx, const void* skip, int Cskip, int N, int H, int W, int Cout, float eps,
+                    const float* norm1_g, const float* norm1_b, const float* conv1_w, const float* conv1_b,
+                    const float* norm2_g, const float* norm2_b, const float* conv2_w, const float* conv2_b,
+                    const float* shortcut_w, const float* shortcut_b, void* y, void* stream);
+/* F.interpolate(x [N,H,W,C], size=(OH,OW)) -> y [N,OH,OW,C]: mode 0 nearest (the UNet's Upsample2D to a skip's size),
+ * 1 bilinear with align_corners=False (the DPT fusion stage's resize of a skip feature).  C % 8 == 0. */
+gp_status gp_resize(int dtype, const void* x, int N, int H, int W, int C, int OH, int OW, int mode, void* y, void* stream);
 /* ---- pre/post-processing around the hot path (SURVEY.md §8 f1); buffers may be host or device ------------
  * gp_resize_aa replaces torchvision.transforms.functional.resize(tensor, size, interpolation, antialias=True)
  * as called by resize_max_res (/root/reference/genpercept/util/image_util.py:75-105) and by the resize back
