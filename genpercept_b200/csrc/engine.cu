@@ -883,6 +883,14 @@ gp_status gp_tile_shape(int cout, int cin, int ks, int images, int h, int w, int
   return GP_OK;
 }
 
+gp_status gp_conv_tile(int cin, int csc, int cout, int images, int h, int w, int num_sms, int* bn, int* mt, int* patch) {
+  if (!bn || !mt || !patch || cin < 1 || csc < 0 || cout < 1 || images < 1 || h < 1 || w < 1 || num_sms < 1) return GP_ERR_INVALID;
+  gp::tile_shape_for(cout, (double)cin * 9 + csc, false, images, w, h, num_sms, bn, mt);
+  const bool staged = cout % 64 == 0 && *bn % 64 == 0;   // Builder::conv: the staged epilogue of a 16-bit NHWC output
+  *patch = staged && gp::patch_tile_fits(images, h, w, cin, csc, cout, *bn, *mt, num_sms) ? 1 : 0;
+  return GP_OK;
+}
+
 gp_status gp_set_timestep(gp_engine* e, int timestep) {
   return guarded(e, [&]() {
     if (!e->finalized) throw GpError(GP_ERR_STATE, "gp_set_timestep before gp_finalize");

@@ -308,5 +308,6 @@ void shared_arena_record(int device, cudaStream_t s);
 // N tile width for a GEMM with `cout` output columns (`force` != 0: that width); one of 16, 32, 64, 128.
 int choose_bn(int cout, int force);
 void tile_shape_for(int cout, double k_elems, bool tokens_mode, int images, int gw, int gh, int num_sms, int* bn, int* mt);
+bool patch_tile_fits(int images, int h, int w, int cin, int csc, int cout, int bn, int mt, int num_sms);
 
 }  // namespace gp

@@ -288,7 +288,7 @@ const char* igemm_finalize(IgemmParams* p) {
     return "staged epilogue needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output, no GEGLU";
   if (p->stats && (!p->tma_store || p->Cout > 512)) return "statistics need the staged epilogue and Cout <= 512";
   // The patch kernel at BN = 128 hands its tile over in two 64-column halves (igemm_common.cuh): a whole 128 x 128 fp32 tile
-  // (64 KiB) next to the two halo patches would leave room for two weight stages only.
+  // (64 KiB) next to the two 30 KiB halo patches and the statistics scratch would cost two of the six weight stages.
   p->acc_half = (p->patch && p->BN == 128) ? 1 : 0;
   if (p->acc_half && (!p->tma_store || p->MT != 1))
     return "patch mode at BN = 128 needs the staged epilogue and MT = 1";
@@ -298,10 +298,20 @@ const char* igemm_finalize(IgemmParams* p) {
   const int fixed = (p->tma_store ? kEpiWarps * 4096 * (p->out_lo ? 2 : 1) : 0) + acc_tile_bytes(*p) + 3072 + stats_bytes;
   const int ring_unit = p->patch ? p->BN * 128 : kABytes * p->MT + p->BN * 128;   // bytes per pipeline stage
   if (p->patch) {
-    if (p->TW != 128 || p->TH != p->MT || p->Z0 != 1 || p->Z1 < 1 || p->nseg[0] != 9 || p->kc_count < 1 ||
-        p->nkb[0] != 9 * p->kc_count || p->npass != 1 || p->gridW % 128 || p->gridH % p->TH || !p->tma_store)
-      return "patch mode needs TW = 128, TH = MT, full tiles, a single-source 3x3 tap table and the staged epilogue";
-    p->a_slot_bytes = ((p->TW + 2) * (p->TH + 2) * 128 + 1023) & ~1023;
+    // nine taps of the main source (map 0), then at most two 1x1 shortcut segments (maps 1, 2: the patch-box views)
+    bool table = p->nseg[0] >= 9 && p->nseg[0] <= 11;
+    int sc_chunks = 0;
+    for (int s = 0; table && s < p->nseg[0]; ++s) {
+      const IgemmSeg& sg = p->seg[0][s];
+      if (s < 9) table = sg.map == 0 && sg.nchunks == p->kc_count && sg.dy == s / 3 - 1 && sg.dx == s % 3 - 1;
+      else table = sg.map == s - 8 && sg.dy == 0 && sg.dx == 0;
+      if (s >= 9) sc_chunks += sg.nchunks;
+    }
+    if (p->TW != kPatchTW || p->TH != 8 * p->MT || p->tw_shift != 4 || p->Z0 != 1 || p->Z1 < 1 || !table || p->kc_count < 1 ||
+        p->nkb[0] != 9 * p->kc_count + sc_chunks || p->npass != 1 || p->gridW % p->TW || p->gridH % p->TH || !p->tma_store)
+      return "patch mode needs 16 x 8 MT tiles that divide the output, a 3x3 tap table of one source (+ up to two 1x1 "
+             "shortcut sources) and the staged epilogue";
+    p->a_slot_bytes = (kPatchPitch * (p->TH + 2) * 128 + 1023) & ~1023;
   }
   const int avail = kMaxSmem - 1024 - fixed - (p->patch ? 2 * p->a_slot_bytes : 0);
   int st = avail / ring_unit;

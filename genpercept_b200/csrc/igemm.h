@@ -22,6 +22,10 @@ constexpr int kMaxSegs = 20;
 constexpr int kMaxClasses = 4;
 constexpr int kBM = 128;      // rows of one accumulator tile (two wgmma m64 blocks)
 constexpr int kBK = 64;       // channels per pipeline stage (= one 128-byte swizzle row of fp16)
+// Patch-resident tiles (igemm_patch.cu): 16 pixels wide, 8 * MT rows high, built from 8 x 8-pixel m64 blocks; the halo
+// patch is loaded kPatchPitch pixels wide (TW + 2 rounded up to a multiple of 8: 8-row core groups 3 KiB apart)
+constexpr int kPatchTW = 16;
+constexpr int kPatchPitch = 24;
 
 struct IgemmSeg {
   int8_t map;        // index into tmA
@@ -88,7 +92,8 @@ struct IgemmParams {
   // shared-memory tile and issues one TMA store (full 128-byte lines, image-edge clipping by the
   // tensor map).  Needs Cout % 64 == 0, BN % 64 == 0, plain 16-bit NHWC output, no GEGLU.  One map per class.
   int tma_store;
-  CUtensorMap tmOut[kMaxClasses];   // (C, W, H, N) views of the output, box (64, min(TW,32), 32/min(TW,32), 1)
+  CUtensorMap tmOut[kMaxClasses];   // (C, W, H, N) views of the output, box (64, min(TW,32), 32/min(TW,32), 1), or (64, 8, 4, 1)
+                                    // for patch tiles (a warp's 32 rows are 8 x 4 pixels of an m64 block: tile_pixel)
   // Residual through TMA (staged epilogue, res1 only): the same boxes of the residual tensor are LOADED into the
   // staging tile before the accumulator is read.  Row-per-thread global loads of a residual cost 32 L1 sector
   // look-ups per warp request.
@@ -100,15 +105,15 @@ struct IgemmParams {
   int acc_half;                  // set by igemm_finalize for the patch kernel at BN = 128: the tile is handed to the epilogue
                                  // in two 64-column halves through a 64-column shared tile (staged epilogue only)
   CUtensorMap tmRes[kMaxClasses];
-  // Patch-resident main loop (igemm_patch.cu; 3x3 stride-1, one source, TW = 128, TH = MT = 1 or 2): per
-  // 64-channel K chunk ONE (TH+2) x (TW+2) halo patch is loaded and all nine taps are fed from it by
-  // row-offset descriptors (tap (dy,dx) starts (h+dy+1)*(TW+2) + dx+1 rows into the patch), instead of
-  // nine shifted boxes.  Cuts the activation L2->SM traffic 9 -> 2.03 reads per element: the narrow-N
-  // (Cout = 128) layers are bound by exactly that traffic (~42 B/clk/SM of unique data).
+  // Patch-resident main loop (igemm_patch.cu; 3x3 stride-1, one main source plus up to two 1x1-shortcut sources, 16 x 8 MT
+  // tiles that divide the output): per 64-channel K chunk ONE (TH+2) x kPatchPitch halo patch is loaded and all nine taps are
+  // fed from it by row-offset descriptors, instead of nine shifted boxes.  The shortcut sources' chunks follow through the
+  // same patch slots (seg[0][9 + j], maps tmA[1 + j] with the patch box) and feed the centre tap only.  Activation L2->SM
+  // traffic drops from 9 to 1.9 (MT = 1) or 1.7 (MT = 2) reads per element.
   int patch;
   int kc_count;                  // 64-channel K chunks per tap (packed weights are tap-major, kc_count*64 wide per tap)
   int a_slot_bytes;              // bytes reserved per patch slot (2 slots), multiple of 1024
-  CUtensorMap tmPatch;           // (C, W, H, N) view of the source, box (64, TW+2, TH+2, 1)
+  CUtensorMap tmPatch;           // (C, W, H, N) view of the main source, box (64, kPatchPitch, TH+2, 1)
 };
 
 cudaError_t igemm_patch_launch(const IgemmParams& p, int grid, cudaStream_t stream);   // igemm_patch.cu

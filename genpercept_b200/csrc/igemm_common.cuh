@@ -52,6 +52,16 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int tile)
   return t;
 }
 
+// Tile row r -> pixel (x, y) inside the tile.  Tap-streaming tiles are TW x TH, row-major; patch-resident tiles are 8 x 8-pixel
+// m64 blocks, TW / 8 of them across (igemm_patch.cu), so a warp's 32 rows there are an 8 x 4-pixel box.
+__device__ __forceinline__ int2 tile_pixel(const IgemmParams& p, int r) {
+  if (p.patch) {
+    const int b = r >> 6, bx_bits = p.tw_shift - 3;
+    return make_int2(((b & ((1 << bx_bits) - 1)) << 3) | (r & 7), ((b >> bx_bits) << 3) | ((r >> 3) & 7));
+  }
+  return make_int2(r & (p.TW - 1), r >> p.tw_shift);
+}
+
 template <bool BF16>
 __device__ __forceinline__ float cvt16(uint16_t v) {
   if constexpr (BF16) {
@@ -266,8 +276,8 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
       const TileCoord tn = decode_tile(p, tile + gridDim.x);
       const int ncls = p.cls_from_z0 ? tn.z0 : 0;
       for (int h = 0; h < p.MT; ++h) {
-        const int r0 = h * 128 + wq * 32;
-        const int psx = tn.tx * p.TW + (r0 & (p.TW - 1)), psy = tn.ty * p.TH + (r0 >> p.tw_shift);
+        const int2 o = tile_pixel(p, h * 128 + wq * 32);
+        const int psx = tn.tx * p.TW + o.x, psy = tn.ty * p.TH + o.y;
         for (int c0 = 0; c0 < p.BN && tn.n_tile * p.BN + c0 < p.Cout; c0 += 64)
           tma_prefetch_l2_4d(&p.tmRes[ncls], tn.n_tile * p.BN + c0, psx, psy, tn.z1);
       }
@@ -282,12 +292,12 @@ __device__ __forceinline__ void epilogue_staged(const IgemmParams& p, uint8_t* s
     for (int h = 0; h < p.MT; ++h) {
       const int r0 = h * 128 + wq * 32;                       // first tile row of this warp
       const int row = r0 + lane;
-      const int ti = row >> p.tw_shift, tj = row & (p.TW - 1);
-      const int gy = t.ty * p.TH + ti, gx = t.tx * p.TW + tj;
+      const int2 tp = tile_pixel(p, row), to = tile_pixel(p, r0);
+      const int gy = t.ty * p.TH + tp.y, gx = t.tx * p.TW + tp.x;
       const bool valid = gy < p.gridH && gx < p.gridW;
       const int oy = gy * p.out_sy + p.cls_py[cls], ox = gx * p.out_sx + p.cls_px[cls];
       const long long pix_off = t.z1 * p.out_z1 + (long long)oy * p.out_row_stride + (long long)ox * p.out_pix_stride;
-      const int sx = t.tx * p.TW + (r0 & (p.TW - 1)), sy = t.ty * p.TH + (r0 >> p.tw_shift);   // store box origin
+      const int sx = t.tx * p.TW + to.x, sy = t.ty * p.TH + to.y;   // store box origin
       for (int c0 = 0; c0 < p.BN; c0 += 64) {
         const int n0 = n_base + c0;
         if (n0 >= p.Cout) {
@@ -508,8 +518,8 @@ __device__ __forceinline__ void epilogue_direct(const IgemmParams& p, float* sbi
     const int bias_origin = p.bias_all ? 0 : n_base;
     for (int h = 0; h < p.MT; ++h) {
       const int row = h * 128 + wq * 32 + lane;
-      const int ti = row >> p.tw_shift, tj = row & (p.TW - 1);
-      const int gy = t.ty * p.TH + ti, gx = t.tx * p.TW + tj;
+      const int2 tp = tile_pixel(p, row);
+      const int gy = t.ty * p.TH + tp.y, gx = t.tx * p.TW + tp.x;
       const bool valid = gy < p.gridH && gx < p.gridW;
       const int oy = gy * p.out_sy + p.cls_py[cls], ox = gx * p.out_sx + p.cls_px[cls];
       const long long pix_off = t.z1 * p.out_z1 + t.z0 * p.out_z0 + (long long)oy * p.out_row_stride +

@@ -1,10 +1,16 @@
-// Patch-resident wgmma implicit GEMM for 3x3 stride-1 convolutions over wide images (W % 128 == 0).
+// Patch-resident wgmma implicit GEMM for 3x3 stride-1 convolutions whose 16 x 8 MT pixel tiles divide the output.
 //
-// Per 64-channel K chunk ONE (TH+2) x 130 pixel halo patch of the source lands in shared memory (a single TMA box,
-// image borders zero-filled) and all nine filter taps are fed from it by row-offset SWIZZLE_128B descriptors: tap
-// (dy,dx) of image row h starts ((h+dy+1)*130 + dx+1) rows into the patch (any 128-byte row is a valid descriptor
-// start because the swizzle is a function of the absolute shared-memory address).
-// Activation traffic L2 -> SM drops from 9 to (TH+2)*130 / (TH*128) reads per element.
+// The M tile is built from 8 x 8-pixel m64 blocks: TW = 16 (two blocks across) by TH = 8 MT (MT blocks down).  Per
+// 64-channel K chunk ONE (TH+2) x kPatchPitch pixel halo patch of the source lands in shared memory (a single TMA box,
+// image borders zero-filled, the columns past TW + 2 over-fetched and never read) and all nine filter taps are fed from it
+// by row-offset SWIZZLE_128B descriptors: core group g (pixel row g) of block (bx, by) for tap (dy, dx) starts at patch row
+// (8 by + g + dy + 1) * kPatchPitch + 8 bx + dx + 1, and the groups are kPatchPitch * 128 bytes apart (a multiple of 1024,
+// so every group has the swizzle phase of the first; any 128-byte row is a valid start because the swizzle is a function
+// of the absolute shared-memory address).  Activation traffic L2 -> SM drops from 9 to 10 * 24 / 128 = 1.9 (MT = 1) or
+// 18 * 24 / 256 = 1.7 (MT = 2) reads per element.
+// A fused 1x1 shortcut (ResNets that change the channel count) is more K chunks: after the nine-tap loop over the main
+// source, each shortcut chunk is loaded through the same patch slots with the same box and feeds the centre tap only; its
+// weights follow the nine taps in the packed matrix.
 //
 // Warp roles (384 threads, 1 CTA / SM, persistent; see igemm_common.cuh): warps 0..3 the staged epilogue, warps 4..7 the
 // wgmma consumer, warp 8 patch producer (two patch slots), warp 11 weight producer (one TMA box per (chunk, tap)).
@@ -15,8 +21,14 @@ namespace gp {
 
 namespace {
 
-constexpr int kPW = kBM + 2;      // patch width in pixels (TW = 128)
-constexpr int kPP = kPW;          // patch row pitch in pixels (one TMA box per patch: rows are contiguous)
+constexpr uint32_t kGroupStride = kPatchPitch * 128;   // bytes between the 8-row core groups of an m64 block
+
+// 64-channel K chunks of the shortcut sources (segments 9.. of the tap table, one per source)
+__device__ __forceinline__ int shortcut_chunks(const IgemmParams& p) {
+  int n = 0;
+  for (int s = 9; s < p.nseg[0]; ++s) n += p.seg[0][s].nchunks;
+  return n;
+}
 
 // K loop of the patch kernel for one (BN, MB = 2 * MT) instance; the whole consumer warpgroup runs it.
 // One batch (the wgmmas of one (chunk, tap)) stays in flight, as in the tap kernel: after batch i is committed and batch
@@ -29,18 +41,20 @@ __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* sm
                                                uint64_t* tempty_bar, int wc, int lane) {
   float d[MB][BN / 2];
   const int b_bytes = BN * 128;
+  const int nchunks = p.kc_count + shortcut_chunks(p);
   int slot = 0, stage = 0;
   uint32_t a_phase = 0, b_phase = 0, acc_phase = 0;
-  // m64 block mb covers image row mb / 2 of the tile, pixels 64 (mb & 1) ..
-  auto row_off = [&](int mb, int dy, int dx) { return ((dy + 1 + (mb >> 1)) * kPP + dx + 1 + (mb & 1) * 64) * 128; };
+  // m64 block mb is the 8 x 8 pixels (bx, by) = (mb & 1, mb >> 1) of the tile; its first row, tap (dy, dx)
+  auto row_off = [&](int mb, int dy, int dx) { return ((8 * (mb >> 1) + dy + 1) * kPatchPitch + 8 * (mb & 1) + dx + 1) * 128; };
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     int held_stage = -1;     // weight stage of the batch in flight
     int held_slot = -1;      // patch slot whose last batch is the one in flight
-    for (int kc = 0; kc < p.kc_count; ++kc) {
+    for (int kc = 0; kc < nchunks; ++kc) {
       mbar_wait(&a_full[slot], a_phase, 3);                                                   // the patch has landed
       const uint32_t patch = smem_u32(smem + slot * p.a_slot_bytes);
-      for (int tap = 0; tap < 9; ++tap) {
-        const int dy = p.seg[0][tap].dy, dx = p.seg[0][tap].dx;
+      const int ntap = kc < p.kc_count ? 9 : 1;                                               // shortcut chunks: centre tap
+      for (int tap = 0; tap < ntap; ++tap) {
+        const int dy = ntap == 9 ? p.seg[0][tap].dy : 0, dx = ntap == 9 ? p.seg[0][tap].dx : 0;
         mbar_wait(&b_full[stage], b_phase, 6);
         const uint64_t b_desc = make_sw128_kmajor_desc(smem_u32(sB + stage * b_bytes));
 #pragma unroll
@@ -48,7 +62,7 @@ __device__ __forceinline__ void patch_consumer(const IgemmParams& p, uint8_t* sm
         wgmma_fence();
 #pragma unroll
         for (int mb = 0; mb < MB; ++mb) {
-          const uint64_t a_desc = make_sw128_kmajor_desc(patch + row_off(mb, dy, dx));
+          const uint64_t a_desc = make_sw128_kmajor_desc(patch + row_off(mb, dy, dx), kGroupStride);
 #pragma unroll
           for (int k = 0; k < kBK / 16; ++k) wgmma_ss<BN, BF16>(d[mb], a_desc + 2 * k, b_desc + 2 * k, (kc | tap | k) ? 1u : 0u);
         }
@@ -120,6 +134,7 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_patch_kernel(const __gr
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmPatch);
+    for (int s = 9; s < p.nseg[0]; ++s) tma_prefetch_desc(&p.tmA[p.seg[0][s].map]);
     tma_prefetch_desc(&p.tmB);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&a_full[i], 1);
@@ -158,43 +173,49 @@ __global__ void __launch_bounds__(kRoleThreads, 1) igemm_patch_kernel(const __gr
   if (warp == 8) {
     // ===================================================================== patch producer
     const bool leader = elect_one();
+    const uint32_t patch_bytes = (uint32_t)((p.TH + 2) * kPatchPitch * 128);
     int slot = 0;
     uint32_t phase = 0;
+    auto load = [&](const CUtensorMap* tm, int k0, int x0, int y0, int z) {
+      mbar_wait(&a_empty[slot], phase ^ 1, 1);
+      if (leader) {
+        mbar_expect_tx(&a_full[slot], patch_bytes);
+        tma_load_4d(smem + slot * p.a_slot_bytes, tm, &a_full[slot], k0, x0, y0, z);
+      }
+      __syncwarp();
+      if (++slot == 2) { slot = 0; phase ^= 1; }
+    };
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile);
       const int x0 = t.tx * p.TW - 1, y0 = t.ty * p.TH - 1;
-      for (int kc = 0; kc < p.kc_count; ++kc) {
-        mbar_wait(&a_empty[slot], phase ^ 1, 1);
-        if (leader) {
-          mbar_expect_tx(&a_full[slot], (uint32_t)((p.TH + 2) * kPW * 128));
-          tma_load_4d(smem + slot * p.a_slot_bytes, &p.tmPatch, &a_full[slot], kc * kBK, x0, y0, t.z1);
-        }
-        __syncwarp();
-        if (++slot == 2) { slot = 0; phase ^= 1; }
-      }
+      for (int kc = 0; kc < p.kc_count; ++kc) load(&p.tmPatch, kc * kBK, x0, y0, t.z1);
+      for (int s = 9; s < p.nseg[0]; ++s)                                     // shortcut sources
+        for (int c = 0; c < p.seg[0][s].nchunks; ++c) load(&p.tmA[p.seg[0][s].map], c * kBK, x0, y0, t.z1);
     }
   } else if (warp == 11) {
     // ===================================================================== weight producer
     const bool leader = elect_one();
+    const int nsc = shortcut_chunks(p);
     int stage = 0;
     uint32_t phase = 0;
+    auto load = [&](int kblk, int b_row) {
+      mbar_wait(&b_empty[stage], phase ^ 1, 5);
+      if (leader) {
+        mbar_expect_tx(&b_full[stage], (uint32_t)b_bytes);
+        tma_load_3d(sB + stage * b_bytes, &p.tmB, &b_full[stage], kblk * kBK, b_row, 0);
+      }
+      __syncwarp();
+      if (++stage == stages) { stage = 0; phase ^= 1; }
+    };
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile);
       const int b_row = t.n_tile * p.BN;
       for (int kc = 0; kc < p.kc_count; ++kc) {
         // kept rolled: unrolled nine times, the default bench.py step ran about 0.2 % slower on an H100 80GB HBM3 (700 W)
 #pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) {
-          const int kblk = tap * p.kc_count + kc;   // packed weights: [tap][chunk]
-          mbar_wait(&b_empty[stage], phase ^ 1, 5);
-          if (leader) {
-            mbar_expect_tx(&b_full[stage], (uint32_t)b_bytes);
-            tma_load_3d(sB + stage * b_bytes, &p.tmB, &b_full[stage], kblk * kBK, b_row, 0);
-          }
-          __syncwarp();
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
+        for (int tap = 0; tap < 9; ++tap) load(tap * p.kc_count + kc, b_row);   // packed weights: [tap][chunk]
       }
+      for (int i = 0; i < nsc; ++i) load(9 * p.kc_count + i, b_row);            // then the shortcut segments
     }
   }
 }

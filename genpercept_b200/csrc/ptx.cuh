@@ -123,16 +123,17 @@ __device__ __forceinline__ void reg_fence(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (rows at 128-byte pitch, 8-row groups
-// 1024 bytes apart).  Bit layout (sm_90): start_address[0,14) (>>4), leading_byte_offset[16,30) (>>4; unused for
-// swizzled K-major, canonical value 1), stride_byte_offset[32,46) (>>4), base_offset[49,52) = 0, layout_type[62,64) = 1
-// (SWIZZLE_128B).  The swizzle is a function of the absolute shared-memory address, so any 128-byte row is a valid start
-// (the patch-resident kernel's tap offsets) and +32 bytes selects the next 16-element K step inside the row.
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (rows at 128-byte pitch, 8-row groups `sbo` bytes apart).
+// Bit layout (sm_90): start_address[0,14) (>>4), leading_byte_offset[16,30) (>>4; unused for swizzled K-major, canonical
+// value 1), stride_byte_offset[32,46) (>>4), base_offset[49,52) = 0, layout_type[62,64) = 1 (SWIZZLE_128B).  The swizzle
+// is a function of the absolute shared-memory address, so any 128-byte row is a valid start (the patch-resident kernel's
+// tap offsets) and +32 bytes selects the next 16-element K step inside the row.  `sbo` must be a multiple of 1024 so that
+// every group starts at the swizzle phase of the first (the patch kernel's groups are patch rows, kPatchPitch * 128 apart).
+__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr, uint32_t sbo = 1024) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
   d |= (uint64_t)1 << 62;
   return d;
 }

@@ -64,6 +64,7 @@ def lib():
     L.gp_shared_arena_info.argtypes = [c_int, POINTER(c_int64), POINTER(c_int64), POINTER(c_int64)]
     L.gp_shared_arena_fill.argtypes = [c_int, c_int, c_void_p]
     L.gp_tile_shape.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]
+    L.gp_conv_tile.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]
     L.gp_tensor_shape.argtypes = [c_void_p, c_char_p, POINTER(c_int64)]
     L.gp_read_tensor.argtypes = [c_void_p, c_char_p, c_void_p, c_size_t]
     L.gp_write_tensor.argtypes = [c_void_p, c_char_p, c_void_p, c_size_t]
@@ -762,6 +763,16 @@ def tile_shape(cout, cin, ks, images, h, w, tokens_mode=False, num_sms=132):
     st = lib().gp_tile_shape(cout, cin, ks, images, h, w, 1 if tokens_mode else 0, num_sms, byref(bn), byref(mt))
     _check_free(st, "gp_tile_shape")
     return bn.value, mt.value
+
+
+def conv_tile(images, h, w, cin, cout, csc=0, num_sms=132):
+    """The tile the planner gives a 3x3 stride-1 convolution in the 16-bit modes (host-only; the rule is Builder::conv in
+    csrc/builder.cu): {"bn", "mt", "patch", "tw", "th"}; tw / th only for the patch-resident kernel (else None)."""
+    bn, mt, patch = c_int(), c_int(), c_int()
+    st = lib().gp_conv_tile(cin, csc, cout, images, h, w, num_sms, byref(bn), byref(mt), byref(patch))
+    _check_free(st, "gp_conv_tile")
+    p = bool(patch.value)
+    return {"bn": bn.value, "mt": mt.value, "patch": p, "tw": 16 if p else None, "th": 8 * mt.value if p else None}
 
 
 def bench_conv(dtype, N, H, W, Cin, Cout, ks=3, mode=0, iters=10):

@@ -117,6 +117,10 @@ gp_status gp_shared_arena_fill(int device, int byte, void* stream);
  * num_sms SMs (tokens_mode != 0: one row of images * h * w tokens).  Nothing in the reference corresponds to it (PyTorch /
  * cuDNN pick their own tiles); it pins the tile policy of tile_shape_for (csrc/builder.cu) in the CPU tests. */
 gp_status gp_tile_shape(int cout, int cin, int ks, int images, int h, int w, int tokens_mode, int num_sms, int* bn, int* mt);
+/* Host-only introspection: the tile the planner gives a 3x3 stride-1 convolution cin -> cout (plus a fused 1x1 shortcut over
+ * csc channels, or 0) over `images` maps of h x w pixels in the 16-bit modes: (BN, MT) as gp_tile_shape, and patch = 1 when
+ * it runs on the patch-resident kernel (16 x 8 MT pixel tiles), 0 for the tap-streaming kernel. */
+gp_status gp_conv_tile(int cin, int csc, int cout, int images, int h, int w, int num_sms, int* bn, int* mt, int* patch);
 /* replaces: the per-call `fix_timesteps` of single_infer (/root/reference/genpercept/genpercept_pipeline.py:405-408).
  * The timestep only enters through conv1.bias + time_emb_proj(silu(emb(t))) of the 22 UNet ResNets; those biases are
  * re-folded on the host (cached per timestep) and rewritten in place after a device synchronisation. */
