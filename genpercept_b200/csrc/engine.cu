@@ -117,13 +117,21 @@ struct Plan {
   // stage, their own first pass, which runs eagerly (kernel attributes, lazy init)
   std::map<std::pair<int, int>, cudaGraphExec_t> graphs;
   std::map<int, int> eager_runs;
+  // gp_infer_steps' whole denoising loops, by (n_steps, noise given, out_channels); each key's first pass runs eagerly
+  std::map<std::tuple<int, int, int>, cudaGraphExec_t> step_graphs;
+  std::map<std::tuple<int, int, int>, int> step_eager_runs;
   double igemm_flops = 0;
   int64_t launches = 0;
 
   Plan() = default;
   Plan(const Plan&) = delete;
   Plan& operator=(const Plan&) = delete;
+  void drop_step_graphs() {
+    for (auto& g : step_graphs) cudaGraphExecDestroy(g.second);
+    step_graphs.clear();
+  }
   ~Plan() {
+    drop_step_graphs();
     for (auto& g : graphs) cudaGraphExecDestroy(g.second);
     if (shared) shared_arena_remove(device, arena_bytes);
     else if (arena) cudaFree(arena);
@@ -142,6 +150,73 @@ struct ArenaUse {
   }
 };
 
+// The UNet's 22 time-embedded ResNets (the conv1 biases a timestep changes) in the order of a step's bias row: down
+// blocks, mid block, up blocks, as unet() emits them.  (name, Cout).
+std::vector<std::pair<std::string, int>> step_bias_layout() {
+  std::vector<std::pair<std::string, int>> l;
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 2; ++j)
+      l.emplace_back("unet.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), kUnetOut[i]);
+  for (int j = 0; j < 2; ++j) l.emplace_back("unet.mid_block.resnets." + std::to_string(j), 1280);
+  const int up_out[4] = {1280, 1280, 640, 320};
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 3; ++j)
+      l.emplace_back("unet.up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), up_out[i]);
+  return l;
+}
+
+// gp_infer_steps' per-step data on the device, one set per engine.  Row i of `table` holds step i's folded conv1 biases
+// in step_bias_layout order (`nbias` floats), then its four DDIM coefficients.  A call folds its rows on the host into
+// the pinned `staging` buffer and uploads them on its stream; before each step's UNet ops, bias_scatter copies that
+// step's row into the live bias buffers (`segs`).  So a captured loop reads the call's timesteps and coefficients as
+// data: nothing in it depends on them.
+struct StepTables {
+  std::vector<std::string> keys;     // the ResNet of each segment
+  std::vector<BiasSegment> host_segs;
+  BiasSegment* segs = nullptr;       // device copy of host_segs
+  int nbias = 0, row = 0;            // floats of biases per step, floats per row (nbias + 4)
+  int cap = 0;                       // rows of `table` and `staging`
+  float* table = nullptr;            // device [cap][row]
+  float* staging = nullptr;          // pinned host [cap][row]
+  cudaEvent_t staged = nullptr;      // recorded after the last upload from `staging`
+  cudaEvent_t released = nullptr;    // recorded after the last call's work: its reads of `table` and the bias buffers,
+                                     // and the hand-off of its result from out_f32
+
+  StepTables() = default;
+  StepTables(const StepTables&) = delete;
+  StepTables& operator=(const StepTables&) = delete;
+  ~StepTables() {
+    if (released) cudaEventSynchronize(released);
+    if (staged) cudaEventSynchronize(staged);
+    if (table) cudaFree(table);
+    if (staging) cudaFreeHost(staging);
+    if (segs) cudaFree(segs);
+    if (staged) cudaEventDestroy(staged);
+    if (released) cudaEventDestroy(released);
+  }
+
+  // Binds the layout to the store's bias buffers (after gp_finalize packed every weight): each of the 22 buffers once.
+  void init(const WeightStore& ws) {
+    int off = 0;
+    for (const auto& [key, cout] : step_bias_layout()) {
+      int rows = 0;
+      float* slot = ws.temb_bias_slot(key, &rows);
+      GP_REQUIRE(slot && rows == cout, key + ": no time-embedded conv1 bias of " + std::to_string(cout) + " channels");
+      keys.push_back(key);
+      host_segs.push_back(BiasSegment{slot, off, cout});
+      off += cout;
+    }
+    GP_REQUIRE(ws.temb_slot_count() == (int)host_segs.size(), "the UNet has time-embedded ResNets outside the step layout");
+    nbias = off;
+    row = nbias + 4;
+    const size_t bytes = host_segs.size() * sizeof(BiasSegment);
+    GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&segs), bytes));
+    GP_CUDA(cudaMemcpy(segs, host_segs.data(), bytes, cudaMemcpyHostToDevice));
+    GP_CUDA(cudaEventCreateWithFlags(&staged, cudaEventDisableTiming));
+    GP_CUDA(cudaEventCreateWithFlags(&released, cudaEventDisableTiming));
+  }
+};
+
 }  // namespace
 
 struct gp_engine {
@@ -156,6 +231,7 @@ struct gp_engine {
   Plan* cur = nullptr;
   bool mem_efficient_attn = false;   // gp_set_memory_efficient_attention: fused attention in the high-precision mode
   bool shared_arena = false;         // gp_set_shared_arena: new plans take their arena from the device's shared pool
+  StepTables steps;                  // the multi-step arch's per-step biases and coefficients (gp_infer_steps)
 
   ~gp_engine() {
     if (!shared_arena) return;
@@ -169,6 +245,26 @@ struct gp_engine {
     GP_CUDA(cudaDeviceSynchronize());
     if (cur == it->second.get()) cur = nullptr;
     plans.erase(it);
+  }
+
+  // Makes room for `n` rows in the step tables.  Growing frees the old table, so the graphs that read it go too; the host
+  // waits only for the last call that used it.
+  void reserve_steps(int n) {
+    StepTables& st = steps;
+    if (n <= st.cap) return;
+    const int cap = std::max(n, 2 * st.cap);
+    GP_CUDA(cudaEventSynchronize(st.released));
+    GP_CUDA(cudaEventSynchronize(st.staged));
+    for (auto& kv : plans) kv.second->drop_step_graphs();
+    if (st.table) GP_CUDA(cudaFree(st.table));
+    if (st.staging) GP_CUDA(cudaFreeHost(st.staging));
+    st.table = nullptr;
+    st.staging = nullptr;
+    st.cap = 0;
+    const size_t bytes = (size_t)cap * st.row * sizeof(float);
+    GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&st.table), bytes));
+    GP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&st.staging), bytes));
+    st.cap = cap;
   }
 
   // ------------------------------------------------------------------ graph pieces
@@ -646,41 +742,82 @@ void stage_rgb(gp_engine* e, Plan* p, const void* rgb, int rgb_dtype, int rgb_on
   GP_CUDA(preprocess_rgb_im2col(src, kind, p->arena + p->rgb.off, p->B, p->H, p->W, e->ws.bf16, s, e->ws.split));
 }
 
+// Whether the plan's passes replay captured graphs: always (use_cuda_graph 1), or with 2 = auto where the launch stream is
+// the bottleneck — small plans.
+bool uses_graph(const gp_engine* e, const Plan* p) {
+  return e->cfg.use_cuda_graph == 1 ||
+         (e->cfg.use_cuda_graph == 2 && (long long)p->B * p->H * p->W <= 2LL * 768 * 768);
+}
+
+// Captures what `enqueue(stream)` launches into an executable graph.
+template <class F>
+cudaGraphExec_t capture_graph(F enqueue) {
+  cudaStream_t cs;
+  GP_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+  cudaGraph_t g;
+  GP_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+  cudaError_t re = enqueue(cs);
+  cudaError_t ce = cudaStreamEndCapture(cs, &g);
+  cudaStreamDestroy(cs);
+  GP_CUDA(re);
+  GP_CUDA(ce);
+  cudaGraphExec_t ge;
+  GP_CUDA(cudaGraphInstantiate(&ge, g, 0));
+  cudaGraphDestroy(g);
+  return ge;
+}
+
 // Runs the ops of stages `first` .. GP_STAGE_READOUT and delivers the result to `out` (device, or host if out_on_host).
 // The first pass from `first` runs eagerly; with CUDA graphs on, later passes replay the graph captured for
 // (first, out_channels).
 void run_to_out(gp_engine* e, Plan* p, int first, float* out, int out_on_host, int out_channels, cudaStream_t s) {
-  // 2 = auto: replay a graph where the launch stream is the bottleneck — small plans
-  const bool use_graph = e->cfg.use_cuda_graph == 1 ||
-                         (e->cfg.use_cuda_graph == 2 && (long long)p->B * p->H * p->W <= 2LL * 768 * 768);
   // eager launches write the result straight into a device `out`; a captured graph has the plan's own buffer baked in
   int& eager_runs = p->eager_runs[first];
-  const bool graph_now = use_graph && eager_runs > 0;
+  const bool graph_now = uses_graph(e, p) && eager_runs > 0;
   ResultTo result(p, (graph_now || out_on_host) ? p->out_f32 : out);
   if (graph_now) {
     const auto key = std::make_pair(first, out_channels);
     auto it = p->graphs.find(key);
-    if (it == p->graphs.end()) {
-      cudaStream_t cs;
-      GP_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-      cudaGraph_t g;
-      GP_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-      cudaError_t re = run_ops(p, first, GP_STAGE_READOUT, out_channels, cs);
-      cudaError_t ce = cudaStreamEndCapture(cs, &g);
-      cudaStreamDestroy(cs);
-      GP_CUDA(re);
-      GP_CUDA(ce);
-      cudaGraphExec_t ge;
-      GP_CUDA(cudaGraphInstantiate(&ge, g, 0));
-      cudaGraphDestroy(g);
-      it = p->graphs.emplace(key, ge).first;
-    }
+    if (it == p->graphs.end())
+      it = p->graphs.emplace(key, capture_graph([&](cudaStream_t cs) { return run_ops(p, first, GP_STAGE_READOUT, out_channels, cs); }))
+               .first;
     GP_CUDA(cudaGraphLaunch(it->second, s));
   } else {
     GP_CUDA(run_ops(p, first, GP_STAGE_READOUT, out_channels, s));
     eager_runs++;
   }
   result.deliver(out, out_on_host, out_channels, s);
+}
+
+// gp_infer_steps from the encode to the readout (genpercept_pipeline.py:416-472), on the plan's fixed buffers: the staged
+// rgb, the noise in out_f32 (when `noise`), and the first n_steps rows of the engine's step tables.  The same launches run
+// eagerly or under capture.
+cudaError_t run_steps(gp_engine* e, Plan* p, int n_steps, bool noise, int out_channels, cudaStream_t s) {
+#define GP_STEP_TRY(call) do { const cudaError_t r__ = (call); if (r__ != cudaSuccess) return r__; } while (0)
+  const WeightStore& ws = e->ws;
+  const StepTables& st = e->steps;
+  GP_STEP_TRY(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, out_channels, s));   // rgb_latent (:416)
+  const T4& lat = p->rgb_latent;
+  const long long npx = lat.pixels();
+  uint8_t* A = p->arena;
+  void* smp = A + p->sample.off;
+  if (noise)                  // marigold: pred_latent = randn (:418-425; the caller draws it with its generator)
+    GP_STEP_TRY(nchw4_affine_to_nhwc8(p->out_f32, smp, lat.N, lat.H, lat.W, 1.0f, nullptr, nullptr, ws.bf16, s, ws.split));
+  else                        // rgb_blending: pred_latent = rgb_latent (:426-427)
+    GP_STEP_TRY(cudaMemcpyAsync(smp, A + lat.off, lat.bytes(), cudaMemcpyDeviceToDevice, s));
+  for (int i = 0; i < n_steps; ++i) {                                                   // :443-463
+    const float* row = st.table + (size_t)i * st.row;
+    GP_STEP_TRY(bias_scatter(row, st.segs, (int)st.host_segs.size(), s));
+    GP_STEP_TRY(latent_pack(A + lat.off, smp, A + p->xin.off, npx, e->unet_in_ch, ws.bf16, s, ws.split));
+    GP_STEP_TRY(run_ops(p, GP_STAGE_UNET, GP_STAGE_UNET, out_channels, s));
+    GP_STEP_TRY(ddim_step(A + p->noise_pred.off, smp, A + p->x0.off, npx, row + st.nbias, ws.bf16, s, ws.split));
+  }
+  // pred_latent = step_output.pred_original_sample (:465); decode_pred (:507-526); clip + shift in the last kernel
+  GP_STEP_TRY(latent_affine(A + p->x0.off, A + p->z.off, npx, 1.0f / kLatentScale, ws.pq_dev, ws.pq_dev + 16, ws.bf16, s,
+                            ws.split));
+  GP_STEP_TRY(run_ops(p, GP_STAGE_READOUT, GP_STAGE_READOUT, out_channels, s));
+  return cudaSuccess;
+#undef GP_STEP_TRY
 }
 
 // gp_encode and gp_encode_exact: the VAE encoder on the caller's rgb; the latent leaves as fp32 [B,4,h,w], or with
@@ -778,6 +915,7 @@ gp_status gp_finalize(gp_engine* e) {
     // A measuring pass over a nominal shape touches every weight the topology needs: packs + uploads.
     Builder b(e->ws.bf16, true, nullptr, e->ws.split);
     e->build(b, nullptr, 1, 64, 64);
+    if (e->multistep) e->steps.init(e->ws);
     e->ws.host.clear();
     e->finalized = true;
   });
@@ -891,6 +1029,20 @@ gp_status gp_conv_tile(int cin, int csc, int cout, int images, int h, int w, int
   return GP_OK;
 }
 
+gp_status gp_step_bias_layout(int capacity, int* n_segments, int* offsets, int* lengths) {
+  if (!n_segments) return GP_ERR_INVALID;
+  const auto layout = step_bias_layout();
+  *n_segments = (int)layout.size();
+  if (capacity < (int)layout.size()) return (offsets || lengths) ? GP_ERR_INVALID : GP_OK;
+  int off = 0;
+  for (size_t k = 0; k < layout.size(); ++k) {
+    if (offsets) offsets[k] = off;
+    if (lengths) lengths[k] = layout[k].second;
+    off += layout[k].second;
+  }
+  return GP_OK;
+}
+
 gp_status gp_set_timestep(gp_engine* e, int timestep) {
   return guarded(e, [&]() {
     if (!e->finalized) throw GpError(GP_ERR_STATE, "gp_set_timestep before gp_finalize");
@@ -974,34 +1126,47 @@ gp_status gp_infer_steps(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_o
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     GP_CUDA(cudaSetDevice(e->cfg.device));
     ArenaUse use(p, s);
-    stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_infer_steps");
-    GP_CUDA(run_ops(p, GP_STAGE_VAE_ENCODE, GP_STAGE_VAE_ENCODE, out_channels, s));      // rgb_latent (:416)
-    const T4& lat = p->rgb_latent;
-    const long long npx = lat.pixels();
-    uint8_t* A = p->arena;
-    void* smp = A + p->sample.off;
-    if (noise) {              // marigold: pred_latent = randn (:418-425; the caller draws it with its generator)
-      const float* nd = noise;
-      if (noise_on_host) {    // the plan's result buffer is free until the decoder runs
-        GP_CUDA(cudaMemcpyAsync(p->out_f32, noise, (size_t)npx * 4 * sizeof(float), cudaMemcpyHostToDevice, s));
-        nd = p->out_f32;
+    StepTables& st = e->steps;
+    e->reserve_steps(n_steps);
+    // Fold this call's rows on the host.  The staging buffer is rewritten only after the previous upload from it is done.
+    GP_CUDA(cudaEventSynchronize(st.staged));
+    for (int i = 0; i < n_steps; ++i) {
+      float* row = st.staging + (size_t)i * st.row;
+      for (size_t k = 0; k < st.keys.size(); ++k) {
+        const std::vector<float>& b = e->ws.temb_bias(timesteps[i], st.keys[k]);
+        std::memcpy(row + st.host_segs[k].off, b.data(), (size_t)st.host_segs[k].len * sizeof(float));
       }
-      GP_CUDA(nchw4_affine_to_nhwc8(nd, smp, lat.N, lat.H, lat.W, 1.0f, nullptr, nullptr, e->ws.bf16, s, e->ws.split));
-    } else {                  // rgb_blending: pred_latent = rgb_latent (:426-427)
-      GP_CUDA(cudaMemcpyAsync(smp, A + lat.off, lat.bytes(), cudaMemcpyDeviceToDevice, s));
+      std::memcpy(row + st.nbias, coeffs + 4 * i, 4 * sizeof(float));
     }
-    for (int i = 0; i < n_steps; ++i) {                                                  // :443-463
-      GP_CUDA(latent_pack(A + lat.off, smp, A + p->xin.off, npx, e->unet_in_ch, e->ws.bf16, s, e->ws.split));
-      e->ws.set_timestep(timesteps[i]);
-      GP_CUDA(run_ops(p, GP_STAGE_UNET, GP_STAGE_UNET, out_channels, s));
-      GP_CUDA(ddim_step(A + p->noise_pred.off, smp, A + p->x0.off, npx, coeffs + 4 * i, e->ws.bf16, s, e->ws.split));
+    // The previous call, on whatever stream, is done with the table, the bias buffers and out_f32 before these land.
+    GP_CUDA(cudaStreamWaitEvent(s, st.released, 0));
+    GP_CUDA(cudaMemcpyAsync(st.table, st.staging, (size_t)n_steps * st.row * sizeof(float), cudaMemcpyHostToDevice, s));
+    GP_CUDA(cudaEventRecord(st.staged, s));
+    stage_rgb(e, p, rgb, rgb_dtype, rgb_on_host, s, "gp_infer_steps");
+    // The caller's noise goes to a fixed buffer, which a graph can read: the plan's result buffer is free until the
+    // decoder runs.
+    if (noise)
+      GP_CUDA(cudaMemcpyAsync(p->out_f32, noise, (size_t)p->rgb_latent.pixels() * 4 * sizeof(float),
+                              noise_on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
+    // As run_to_out: the first pass of a key runs eagerly, later ones replay its graph, which writes out_f32.
+    const auto key = std::make_tuple(n_steps, noise ? 1 : 0, out_channels);
+    int& eager_runs = p->step_eager_runs[key];
+    const bool graph_now = uses_graph(e, p) && eager_runs > 0;
+    ResultTo result(p, (graph_now || out_on_host) ? p->out_f32 : out);
+    if (graph_now) {
+      auto it = p->step_graphs.find(key);
+      if (it == p->step_graphs.end())
+        it = p->step_graphs
+                 .emplace(key, capture_graph([&](cudaStream_t cs) { return run_steps(e, p, n_steps, noise != nullptr, out_channels, cs); }))
+                 .first;
+      GP_CUDA(cudaGraphLaunch(it->second, s));
+    } else {
+      GP_CUDA(run_steps(e, p, n_steps, noise != nullptr, out_channels, s));
+      eager_runs++;
     }
-    // pred_latent = step_output.pred_original_sample (:465); decode_pred (:507-526); clip + shift in the last kernel
-    GP_CUDA(latent_affine(A + p->x0.off, A + p->z.off, npx, 1.0f / kLatentScale, e->ws.pq_dev, e->ws.pq_dev + 16,
-                          e->ws.bf16, s, e->ws.split));
-    ResultTo result(p, out_on_host ? p->out_f32 : out);
-    GP_CUDA(run_ops(p, GP_STAGE_READOUT, GP_STAGE_READOUT, out_channels, s));
+    e->ws.cur_timestep = timesteps[n_steps - 1];     // the bias buffers hold the last step's values
     result.deliver(out, out_on_host, out_channels, s);
+    GP_CUDA(cudaEventRecord(st.released, s));
     if (rgb_on_host || out_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }

@@ -217,7 +217,7 @@ class WeightStore {
   int n_tokens = 0;
   size_t weight_bytes = 0;
   float* pq_dev = nullptr;   // vae.post_quant_conv: [16] weight + [4] bias, fp32 on the device
-  int cur_timestep = 0;
+  int cur_timestep = 0;      // the timestep whose biases the live conv1 bias slots hold once the queued work has run
 
   void put(const std::string& key, std::vector<int64_t> shape, const float* d);
   template <class Tp>
@@ -258,12 +258,19 @@ class WeightStore {
 
   void compute_temb(int timestep);
   void set_timestep(int timestep);
+  // The live conv1 bias buffer (rows() floats) of time-embedded ResNet `p`, or null when `p` has none.
+  float* temb_bias_slot(const std::string& p, int* rows) const;
+  // The number of time-embedded ResNets packed so far.
+  int temb_slot_count() const { return (int)temb_layers.size(); }
+  // conv1.bias + time_emb_proj(silu(emb(timestep))) of ResNet `p`, the value set_timestep writes (cached per timestep).
+  const std::vector<float>& temb_bias(int timestep, const std::string& p);
 
  private:
   const HostT& T(const std::string& k) const;
   bool has(const std::string& k) const { return host.count(k) != 0; }
   void upload_post_quant();
   std::vector<float> temb_for(int timestep) const;
+  const std::vector<std::vector<float>>& temb_biases(int timestep);
 
   std::vector<void*> dev_allocs;
   std::unordered_map<std::string, PackedW> packed;
@@ -275,7 +282,7 @@ class WeightStore {
   // Per-call fix_timesteps (genpercept_pipeline.py:405-408): the timestep only enters through
   // conv1.bias + time_emb_proj(silu(emb(t))) of the 22 UNet ResNets, so changing it re-folds those biases in place
   // (the device bias buffers keep their addresses: every plan and captured graph sees the new values).
-  struct TembLayer { std::vector<float> w, b, conv_bias; float* dev_bias = nullptr; int cout = 0; };
+  struct TembLayer { std::string key; std::vector<float> w, b, conv_bias; float* dev_bias = nullptr; int cout = 0; };
   std::vector<TembLayer> temb_layers;
   std::vector<float> te_w1, te_b1, te_w2, te_b2;
   std::map<int, std::vector<std::vector<float>>> temb_cache;   // timestep -> folded bias per layer

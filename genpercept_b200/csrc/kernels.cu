@@ -1079,9 +1079,10 @@ __global__ void latent_pack_kernel(const uint16_t* __restrict__ lat, const uint1
 // (genpercept_b200/scheduler.py step_coefficients); prev_sample overwrites `smp`.
 template <bool BF16>
 __global__ void ddim_step_kernel(const uint16_t* __restrict__ mo, uint16_t* __restrict__ smp, uint16_t* __restrict__ x0, long long npx,
-                                 float c0, float c1, float c2, float c3, int lo) {
+                                 const float* __restrict__ c, int lo) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npx) return;
+  const float c0 = c[0], c1 = c[1], c2 = c[2], c3 = c[3];
   const long long o = i * (lo ? 16 : 8);
   float m[8], x[8], p0[8], pv[8];
   load8<BF16>(mo + o, lo, m);
@@ -1112,7 +1113,16 @@ __global__ void latent_affine_kernel(const uint16_t* __restrict__ in, uint16_t* 
   }
   store8<BF16>(out + o, lo, f);
 }
+__global__ void bias_scatter_kernel(const float* __restrict__ row, const BiasSegment* __restrict__ segs) {
+  const BiasSegment sg = segs[blockIdx.x];
+  for (int i = threadIdx.x; i < sg.len; i += blockDim.x) sg.dst[i] = row[sg.off + i];
+}
 }  // namespace
+
+cudaError_t bias_scatter(const float* row, const BiasSegment* segs, int nseg, cudaStream_t s) {
+  launch(bias_scatter_kernel, (unsigned)nseg, 256, 0, s, row, segs);
+  return cudaGetLastError();
+}
 
 cudaError_t latent_pack(const void* lat, const void* smp, void* xin, long long npx, int in_ch, bool bf16, cudaStream_t s, bool split) {
   GP_DISPATCH_BF16(bf16, (launch(latent_pack_kernel<BF>, (unsigned)((npx + 255) / 256), 256, 0, s, 
@@ -1120,10 +1130,10 @@ cudaError_t latent_pack(const void* lat, const void* smp, void* xin, long long n
                              reinterpret_cast<uint16_t*>(xin), npx, in_ch, split ? 8 : 0)));
   return cudaGetLastError();
 }
-cudaError_t ddim_step(const void* model_out, void* sample, void* x0, long long npx, const float c[4], bool bf16, cudaStream_t s, bool split) {
-  GP_DISPATCH_BF16(bf16, (launch(ddim_step_kernel<BF>, (unsigned)((npx + 255) / 256), 256, 0, s, 
+cudaError_t ddim_step(const void* model_out, void* sample, void* x0, long long npx, const float* c_dev, bool bf16, cudaStream_t s, bool split) {
+  GP_DISPATCH_BF16(bf16, (launch(ddim_step_kernel<BF>, (unsigned)((npx + 255) / 256), 256, 0, s,
                              reinterpret_cast<const uint16_t*>(model_out), reinterpret_cast<uint16_t*>(sample),
-                             reinterpret_cast<uint16_t*>(x0), npx, c[0], c[1], c[2], c[3], split ? 8 : 0)));
+                             reinterpret_cast<uint16_t*>(x0), npx, c_dev, split ? 8 : 0)));
   return cudaGetLastError();
 }
 cudaError_t latent_affine(const void* in, void* out, long long npx, float pre, const float* mat, const float* bias, bool bf16,

@@ -105,10 +105,15 @@ inline int im2col_tap_slot(int r, int q) {      // 3x3 tap (r, q) -> group of 3 
   return lin < 4 ? lin + 1 : lin;
 }
 // Multi-step archs (SURVEY.md §8 f4), 16-bit NHWC8 latents: the UNet input of a step (in_ch 8: [rgb_latent | pred_latent],
-// 4: pred_latent), the DDIM update (eta = 0; coefficients from genpercept_b200/scheduler.py) and post_quant_conv(x / 0.18215).
+// 4: pred_latent), the DDIM update (eta = 0; coefficients from genpercept_b200/scheduler.py, read from the device array
+// c_dev[4]) and post_quant_conv(x / 0.18215).
 cudaError_t latent_pack(const void* lat, const void* smp, void* xin, long long npx, int in_ch, bool bf16, cudaStream_t s, bool split = false);
-cudaError_t ddim_step(const void* model_out, void* sample, void* x0, long long npx, const float c[4], bool bf16, cudaStream_t s,
+cudaError_t ddim_step(const void* model_out, void* sample, void* x0, long long npx, const float* c_dev, bool bf16, cudaStream_t s,
                       bool split = false);
+// One step's row of the multi-step bias table into the UNet's live conv1 bias buffers: segment k copies len floats from
+// row + off to dst.  segs (device) holds nseg segments; one block per segment.
+struct BiasSegment { float* dst; int off; int len; };
+cudaError_t bias_scatter(const float* row, const BiasSegment* segs, int nseg, cudaStream_t s);
 cudaError_t latent_affine(const void* in, void* out, long long npx, float pre, const float* mat, const float* bias, bool bf16,
                           cudaStream_t s, bool split = false);
 // per-image (x - min) / (max - min) over HW fp32 values, in place; scratch: 2 uint32 per image.

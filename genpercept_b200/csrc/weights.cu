@@ -359,6 +359,7 @@ const PackedW& WeightStore::resnet_conv1(const std::string& p, int cin, bool tem
   if (it != packed.end()) return it->second;
   if (!temb_on) return conv_w(p + ".conv1", {cin});
   TembLayer tl;
+  tl.key = p;
   tl.w = T(p + ".time_emb_proj.weight").d;
   tl.b = T(p + ".time_emb_proj.bias").d;
   tl.conv_bias = T(p + ".conv1.bias").d;
@@ -555,9 +556,9 @@ std::vector<float> WeightStore::temb_for(int timestep) const {
   return temb;
 }
 
-void WeightStore::set_timestep(int timestep) {
+// The folded conv1 bias of every time-embedded ResNet at `timestep`, in temb_layers order, computed once per timestep.
+const std::vector<std::vector<float>>& WeightStore::temb_biases(int timestep) {
   GP_REQUIRE(timestep >= 0 && timestep <= 1000, "gp_set_timestep: timestep must be in [0, 1000]");
-  if (timestep == cur_timestep) return;
   auto it = temb_cache.find(timestep);
   if (it == temb_cache.end()) {
     const std::vector<float> emb = temb_for(timestep);
@@ -570,9 +571,29 @@ void WeightStore::set_timestep(int timestep) {
     });
     it = temb_cache.emplace(timestep, std::move(biases)).first;
   }
+  return it->second;
+}
+
+float* WeightStore::temb_bias_slot(const std::string& p, int* rows) const {
+  for (const auto& tl : temb_layers)
+    if (tl.key == p) { *rows = tl.cout; return tl.dev_bias; }
+  return nullptr;
+}
+
+const std::vector<float>& WeightStore::temb_bias(int timestep, const std::string& p) {
+  const auto& biases = temb_biases(timestep);
+  for (size_t i = 0; i < temb_layers.size(); ++i)
+    if (temb_layers[i].key == p) return biases[i];
+  throw GpError(GP_ERR_STATE, p + " has no time-embedded bias");
+}
+
+void WeightStore::set_timestep(int timestep) {
+  GP_REQUIRE(timestep >= 0 && timestep <= 1000, "gp_set_timestep: timestep must be in [0, 1000]");
+  if (timestep == cur_timestep) return;
+  const auto& biases = temb_biases(timestep);
   GP_CUDA(cudaDeviceSynchronize());          // nothing in flight may still read the old biases
   for (size_t i = 0; i < temb_layers.size(); ++i)
-    GP_CUDA(cudaMemcpy(temb_layers[i].dev_bias, it->second[i].data(), (size_t)temb_layers[i].cout * 4, cudaMemcpyHostToDevice));
+    GP_CUDA(cudaMemcpy(temb_layers[i].dev_bias, biases[i].data(), (size_t)temb_layers[i].cout * 4, cudaMemcpyHostToDevice));
   cur_timestep = timestep;
 }
 

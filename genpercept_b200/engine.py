@@ -55,6 +55,7 @@ def lib():
     L.gp_encode_exact.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
     L.gp_infer_latent.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]
     L.gp_set_timestep.argtypes = [c_void_p, c_int]
+    L.gp_step_bias_layout.argtypes = [c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]
     L.gp_infer_steps.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, POINTER(c_int), POINTER(c_float), c_int, c_void_p,
                                  c_int, c_int, c_void_p]
     L.gp_ensemble_reduce.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
@@ -309,7 +310,9 @@ class Engine:
 
     def infer_steps(self, rgb, timesteps, coeffs, noise=None, out_channels=1, out=None):
         """Multi-step archs (gp_infer_steps): `timesteps` [n] ints, `coeffs` [n,4] DDIM coefficients
-        (scheduler.DDIMSchedule.step_coefficients), `noise` fp32 [B,4,h,w] (marigold) or None (rgb_blending)."""
+        (scheduler.DDIMSchedule.step_coefficients), `noise` fp32 [B,4,h,w] (marigold) or None (rgb_blending).
+        Stream-ordered on the current stream: with cuda `rgb`, `noise` and `out` it returns before the GPU finishes.
+        With graphs on, each (n, noise or not, out_channels) runs eagerly once, then replays one graph of the loop."""
         assert rgb.dim() == 4 and rgb.shape[1] == 3
         B, _, H, W = rgb.shape
         self._plan_for(B, H, W)
@@ -763,6 +766,16 @@ def tile_shape(cout, cin, ks, images, h, w, tokens_mode=False, num_sms=132):
     st = lib().gp_tile_shape(cout, cin, ks, images, h, w, 1 if tokens_mode else 0, num_sms, byref(bn), byref(mt))
     _check_free(st, "gp_tile_shape")
     return bn.value, mt.value
+
+
+def step_bias_layout():
+    """The row layout of gp_infer_steps' per-step bias table (host-only): [(offset, length)] in floats, one segment per
+    time-embedded UNet ResNet, in the order down blocks, mid block, up blocks."""
+    n = c_int()
+    _check_free(lib().gp_step_bias_layout(0, byref(n), None, None), "gp_step_bias_layout")
+    off, ln = (c_int * n.value)(), (c_int * n.value)()
+    _check_free(lib().gp_step_bias_layout(n.value, byref(n), off, ln), "gp_step_bias_layout")
+    return list(zip(off, ln))
 
 
 def conv_tile(images, h, w, cin, cout, csc=0, num_sms=132):

@@ -26,6 +26,19 @@ from .engine import Engine
 from .image_util import _lut, get_tv_resample_method, resize_max_res
 
 ONE_CHANNEL_MODES = ("depth", "matting", "dis", "disparity")     # genpercept_pipeline.py:523
+_NO_SCHEDULER = "the multi-step archs need a scheduler (hf_configs/scheduler_beta_*/scheduler_config.json)"
+
+
+def _checkpoint_scheduler(root, kw):
+    """diffusers' from_pretrained loads ``<root>/scheduler/`` when no scheduler is passed: the multi-step archs
+    (genpercept_pipeline=False) take the folder's scheduler_config.json, as run.py's default invocation expects
+    (run.py:361-368).  A missing file raises the ValueError of a missing scheduler, naming the path."""
+    if kw.get("genpercept_pipeline", True) or kw.get("scheduler") is not None:
+        return
+    path = os.path.join(str(root), "scheduler", "scheduler_config.json")
+    if not os.path.isfile(path):
+        raise ValueError(f"{_NO_SCHEDULER}: {path} does not exist")
+    kw["scheduler"] = path
 
 
 @dataclass
@@ -98,14 +111,20 @@ class GenPerceptPipeline:
             # multi-step archs (run.py --archs marigold / rgb_blending, SURVEY.md §8 f4): real DDIM steps around the UNet.
             # `scheduler`: a scheduler_config.json path / folder / dict, a DDIMSchedule, or any object whose .config
             # carries the reference's scheduler fields (the reference passes its DDIMSchedulerCustomized).
-            from .scheduler import DDIMSchedule
+            # The scheduler must be a DDIM one (scheduler.check_scheduler_class): the config's _class_name, else the
+            # object's class name.
+            from .scheduler import DDIMSchedule, check_scheduler_class
             if customized_head is not None:
                 raise ValueError("the DPT readout is one-step (genpercept_pipeline.py:474-483)")
             if scheduler is None:
-                raise ValueError("the multi-step archs need a scheduler (hf_configs/scheduler_beta_*/scheduler_config.json)")
+                raise ValueError(_NO_SCHEDULER)
             if not isinstance(scheduler, DDIMSchedule):
                 cfg = getattr(scheduler, "config", scheduler)
-                scheduler = DDIMSchedule.from_config(dict(cfg) if not isinstance(cfg, (str, os.PathLike)) else cfg)
+                if not isinstance(cfg, (str, os.PathLike)):
+                    cfg = dict(cfg)
+                    if not isinstance(scheduler, dict) and cfg.get("_class_name") is None:
+                        check_scheduler_class(type(scheduler).__name__)
+                scheduler = DDIMSchedule.from_config(cfg)
         self.scheduler = scheduler
         self.text_encoder = text_encoder
         self.tokenizer = tokenizer
@@ -144,8 +163,10 @@ class GenPerceptPipeline:
     def from_pretrained(cls, pretrained_model_name_or_path, variant=None, torch_dtype=None, **kw):
         """Mirrors ``GenPerceptPipeline.from_pretrained(sd21_dir, variant=…, torch_dtype=…,
         genpercept_pipeline=True, unet=…, scheduler=…, [customized_head|vae]=…)`` (run.py:374-376):
-        vae / text_encoder / tokenizer come from the SD-2.1 folder unless passed."""
+        vae / text_encoder / tokenizer come from the SD-2.1 folder unless passed, and so does the scheduler
+        (``scheduler/scheduler_config.json``) of the multi-step archs (genpercept_pipeline=False)."""
         root = str(pretrained_model_name_or_path)
+        _checkpoint_scheduler(root, kw)
         if kw.get("vae") is None:
             kw["vae"] = os.path.join(root, "vae")
         if kw.get("unet") is None:
@@ -163,6 +184,7 @@ class GenPerceptPipeline:
         ``dpt_head_identity/`` or ``vae_decoder/`` + ``vae_post_quant_conv/`` next to it) and ``--lora_rank``.
         See genpercept_b200/loader.py for the layouts."""
         from . import loader
+        _checkpoint_scheduler(checkpoint, kw)
         parts = loader.assemble(checkpoint, unet=unet, lora_rank=lora_rank, variant=kw.get("variant"))
         root = str(checkpoint)
         if kw.get("text_embed") is None and kw.get("text_encoder") is None and os.path.isdir(os.path.join(root, "text_encoder")):

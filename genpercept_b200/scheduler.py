@@ -17,6 +17,17 @@ import os
 
 import numpy as np
 
+# The scheduler classes whose step this module restates: diffusers' DDIMScheduler and the reference's subclass of it.
+DDIM_CLASSES = ("DDIMScheduler", "DDIMSchedulerCustomized")
+
+
+def check_scheduler_class(name):
+    """Raises NotImplementedError unless `name` (a config's ``_class_name`` or a scheduler object's class name) is one of
+    DDIM_CLASSES; None (a config that names no class) passes."""
+    if name is not None and name not in DDIM_CLASSES:
+        raise NotImplementedError(f"scheduler class {name!r} is not supported: the multi-step archs run DDIM steps "
+                                  f"({' or '.join(DDIM_CLASSES)})")
+
 
 class DDIMSchedule:
     def __init__(self, num_train_timesteps=1000, beta_start=0.0001, beta_end=0.02, beta_schedule="linear",
@@ -52,7 +63,8 @@ class DDIMSchedule:
 
     @classmethod
     def from_config(cls, path_or_dict):
-        """A ``scheduler_config.json`` file, the folder holding one, or the parsed dict."""
+        """A ``scheduler_config.json`` file, the folder holding one, or the parsed dict.  Its ``_class_name``, when
+        given, must be a DDIM class (check_scheduler_class)."""
         cfg = path_or_dict
         if not isinstance(cfg, dict):
             p = str(path_or_dict)
@@ -60,6 +72,7 @@ class DDIMSchedule:
                 p = os.path.join(p, "scheduler_config.json")
             with open(p) as f:
                 cfg = json.load(f)
+        check_scheduler_class(cfg.get("_class_name"))
         return cls(**{k: v for k, v in cfg.items() if not k.startswith("_")})
 
     def set_timesteps(self, num_inference_steps, device=None):

@@ -125,6 +125,10 @@ gp_status gp_conv_tile(int cin, int csc, int cout, int images, int h, int w, int
  * The timestep only enters through conv1.bias + time_emb_proj(silu(emb(t))) of the 22 UNet ResNets; those biases are
  * re-folded on the host (cached per timestep) and rewritten in place after a device synchronisation. */
 gp_status gp_set_timestep(gp_engine* e, int timestep);
+/* Host-only: the layout of one step's row of gp_infer_steps' bias table, one segment per time-embedded UNet ResNet
+ * (down blocks, mid block, up blocks): its offset and length in floats.  *n_segments gets the count (22); offsets and
+ * lengths (nullable) need `capacity` >= that count. */
+gp_status gp_step_bias_layout(int capacity, int* n_segments, int* offsets, int* lengths);
 
 /* replaces: single_infer.  rgb: [B,3,H,W] NCHW, device (or pinned/pageable host if
  * rgb_on_host != 0; copied on `stream`), dtype GP_U8 (0..255, mapped x/255*2-1 as
@@ -163,7 +167,13 @@ gp_status gp_infer_latent(gp_engine* e, const float* latent_dev, int batch, int 
  *   rgb_latent = encode_rgb(rgb); pred_latent = noise (marigold; fp32 [B,4,h,w], host or device) or rgb_latent (noise == NULL:
  *   rgb_blending); per step i: unet(cat([rgb_latent, pred_latent]) or pred_latent, timesteps[i]) -> DDIM step with
  *   coeffs[4 i .. 4 i + 3] = (x0 <- sample, x0 <- model_output, prev <- sample, prev <- model_output) (eta = 0; host
- *   arrays, genpercept_b200/scheduler.py); then decode_pred(pred_original_sample), clip, shift.  out as for gp_infer. */
+ *   arrays, genpercept_b200/scheduler.py); then decode_pred(pred_original_sample), clip, shift.  out as for gp_infer.
+ * Each step's conv1 biases (folded on the host, cached per timestep) and coefficients are uploaded with the call on
+ * `stream` and copied into place on the device before the step, so no host or device synchronisation runs between
+ * steps.  With CUDA graphs on (gp_config.use_cuda_graph, the same rule as gp_infer), the first call for each
+ * (n_steps, noise given or not, out_channels) runs eagerly and later calls replay one graph of the whole loop, encode to
+ * readout.  Asynchronous on `stream` unless a host buffer is involved, in which case it returns after the copy.  After the
+ * call the UNet holds the last step's timestep (as gp_set_timestep(timesteps[n_steps - 1]) would leave it). */
 gp_status gp_infer_steps(gp_engine* e, const void* rgb, int rgb_dtype, int rgb_on_host, const float* noise, int noise_on_host,
                          const int* timesteps, const float* coeffs, int n_steps, float* out, int out_on_host, int out_channels,
                          void* stream);
