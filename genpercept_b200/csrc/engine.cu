@@ -93,6 +93,67 @@ void geglu_projection(Builder& b, WeightStore& ws, const std::string& blk, const
   b.conv(blk + ".ff.proj_geglu", c);
 }
 
+// transformers' CLIPTextTransformer.forward with causal masking and no padding mask (the reference tokenizes with
+// padding='do_not_pad'): genpercept_pipeline.py:360-372
+void text_tower(Builder& b, WeightStore& ws, int n, const int32_t* ids, float* out) {
+  GP_REQUIRE(n >= 1 && n <= kTextMaxTokens, "text tower: 1 to " + std::to_string(kTextMaxTokens) + " tokens");
+  const int D = kTextDim;
+  const std::string m = "text.text_model.";
+  const bool bf = b.bf16(), sp = b.split();
+  const float* tok = ws.f32_w(m + "embeddings.token_embedding.weight");
+  const float* pos = ws.f32_w(m + "embeddings.position_embedding.weight");
+  T4 x = b.alloc(1, 1, n, D);
+  if (!b.measuring()) {
+    void* xp = b.ptr(x);
+    b.custom(m + "embeddings", 1, (double)n * D * 8 + (double)x.bytes(),
+             [=](cudaStream_t s) { return text_embed(ids, n, tok, pos, xp, D, bf, s, sp); });
+  }
+  for (int i = 0; i < kTextLayers; ++i) {
+    const std::string p = m + "encoder.layers." + std::to_string(i);
+    T4 l = b.alloc(1, 1, n, D);
+    b.ln(p + ".layer_norm1", x, ws.norm_w(p + ".layer_norm1"), 1e-5f, l);
+    T4 qkv = b.alloc(1, 1, n, 3 * D);
+    { ConvArgs c; c.srcs = {l}; c.ks = 1; c.w = &ws.text_qkv_w(p + ".self_attn"); c.out = qkv; b.conv(p + ".self_attn.qkv", c); }
+    b.release(l);
+    T4 a = b.alloc(1, 1, n, D);
+    if (!b.measuring()) {
+      const void* qp = b.ptr(qkv);
+      void* ap = b.ptr(a);
+      b.custom(p + ".self_attn.causal", 1, (double)qkv.bytes() + (double)a.bytes(),
+               [=](cudaStream_t s) { return causal_attention(qp, n, kTextHeads, D / kTextHeads, ap, bf, s, sp); });
+    }
+    b.release(qkv);
+    T4 x1 = b.alloc(1, 1, n, D);
+    { ConvArgs c; c.srcs = {a}; c.ks = 1; c.w = &ws.lin_w(p + ".self_attn.out_proj"); c.out = x1; c.res1 = &x; b.conv(p + ".self_attn.out_proj", c); }
+    b.release(a);
+    b.release(x);
+    l = b.alloc(1, 1, n, D);
+    b.ln(p + ".layer_norm2", x1, ws.norm_w(p + ".layer_norm2"), 1e-5f, l);
+    T4 h = b.alloc(1, 1, n, kTextMlp);
+    { ConvArgs c; c.srcs = {l}; c.ks = 1; c.w = &ws.lin_w(p + ".mlp.fc1"); c.out = h; b.conv(p + ".mlp.fc1", c); }
+    b.release(l);
+    T4 g = b.alloc(1, 1, n, kTextMlp);
+    if (!b.measuring()) {
+      const void* hp = b.ptr(h);
+      void* gq = b.ptr(g);
+      b.custom(p + ".mlp.gelu", 1, 2.0 * h.bytes(),
+               [=](cudaStream_t s) { return gelu16(hp, gq, (long long)n * kTextMlp, bf, s, sp ? kTextMlp : 0); });
+    }
+    b.release(h);
+    x = b.alloc(1, 1, n, D);
+    { ConvArgs c; c.srcs = {g}; c.ks = 1; c.w = &ws.lin_w(p + ".mlp.fc2"); c.out = x; c.res1 = &x1; b.conv(p + ".mlp.fc2", c); }
+    b.release(g);
+    b.release(x1);
+  }
+  const NormW& fn = ws.norm_w(m + "final_layer_norm");
+  if (!b.measuring()) {
+    const void* xp = b.ptr(x);
+    b.custom(m + "final_layer_norm", 1, (double)x.bytes() + (double)n * D * 4,
+             [=](cudaStream_t s) { return layernorm_f32(xp, out, n, D, fn.gamma, fn.beta, 1e-5f, bf, s, sp); });
+  }
+  b.release(x);
+}
+
 }  // namespace gp
 
 namespace {
@@ -217,6 +278,51 @@ struct StepTables {
   }
 };
 
+// gp_encode_text's tower for one token count: its own arena (the ids, the fp32 result, then the activations) and ops.
+struct TextPlan {
+  uint8_t* arena = nullptr;
+  int32_t* ids = nullptr;
+  float* out = nullptr;
+  std::vector<Op> ops;
+  TextPlan() = default;
+  TextPlan(const TextPlan&) = delete;
+  TextPlan& operator=(const TextPlan&) = delete;
+  ~TextPlan() { if (arena) cudaFree(arena); }
+};
+
+// The text tower of an engine until gp_finalize: the text.* checkpoint tensors, the device weights packed from them (a
+// store of its own, outside the image plans' weight bytes) and a plan per token count.
+struct TextTower {
+  std::unique_ptr<WeightStore> ws;
+  std::map<int, std::unique_ptr<TextPlan>> plans;
+  bool packed = false;        // ws holds device weights
+
+  // The plan for n tokens: the measuring pass sizes the arena (and packs the weights on first use), the second emits.
+  TextPlan* plan(int n) {
+    auto it = plans.find(n);
+    if (it != plans.end()) return it->second.get();
+    auto emit = [&](Builder& b, TextPlan* p) {
+      const size_t ids_off = b.raw_alloc((size_t)kTextMaxTokens * sizeof(int32_t));
+      const size_t out_off = b.raw_alloc((size_t)n * kTextDim * sizeof(float));
+      if (p) {
+        p->ids = reinterpret_cast<int32_t*>(b.raw_ptr(ids_off));
+        p->out = reinterpret_cast<float*>(b.raw_ptr(out_off));
+      }
+      text_tower(b, *ws, n, p ? p->ids : nullptr, p ? p->out : nullptr);
+    };
+    Builder m(ws->bf16, true, nullptr, ws->split);
+    packed = true;
+    emit(m, nullptr);
+    std::unique_ptr<TextPlan> p(new TextPlan());
+    GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->arena), m.arena_bytes()));
+    Builder b(ws->bf16, false, p->arena, ws->split);
+    emit(b, p.get());
+    if (b.arena_bytes() != m.arena_bytes()) throw GpError(GP_ERR_STATE, "text tower: planner passes disagree on arena size");
+    p->ops = std::move(b.ops);
+    return plans.emplace(n, std::move(p)).first->second.get();
+  }
+};
+
 }  // namespace
 
 struct gp_engine {
@@ -232,6 +338,7 @@ struct gp_engine {
   bool mem_efficient_attn = false;   // gp_set_memory_efficient_attention: fused attention in the high-precision mode
   bool shared_arena = false;         // gp_set_shared_arena: new plans take their arena from the device's shared pool
   StepTables steps;                  // the multi-step arch's per-step biases and coefficients (gp_infer_steps)
+  TextTower text;                    // gp_encode_text until gp_finalize
 
   ~gp_engine() {
     if (!shared_arena) return;
@@ -885,6 +992,16 @@ gp_status gp_load_tensor(gp_engine* e, const char* key, const void* host_ptr, in
   return guarded(e, [&]() {
     GP_REQUIRE(key && host_ptr && shape && ndim >= 1 && ndim <= 4, "gp_load_tensor: bad arguments");
     if (e->finalized) throw GpError(GP_ERR_STATE, "gp_load_tensor after gp_finalize");
+    const bool text = std::strncmp(key, "text.", 5) == 0;
+    if (text) {
+      if (std::strcmp(key, "text.text_model.embeddings.position_ids") == 0) return;   // a buffer of arange(77)
+      const auto& spec = text_tower_spec();
+      auto it = spec.find(key);
+      GP_REQUIRE(it != spec.end(), std::string("gp_load_tensor: ") + key + " is not a tensor of SD-2.1's CLIP text tower");
+      GP_REQUIRE(std::vector<int64_t>(shape, shape + ndim) == it->second,
+                 std::string("gp_load_tensor: ") + key + " does not have the shape of SD-2.1's CLIP text tower (d = 1024, "
+                 "23 layers, MLP 4096, vocabulary 49408)");
+    }
     HostT t;
     t.shape.assign(shape, shape + ndim);
     const int64_t n = t.numel();
@@ -894,7 +1011,42 @@ gp_status gp_load_tensor(gp_engine* e, const char* key, const void* host_ptr, in
       const uint16_t* s = reinterpret_cast<const uint16_t*>(host_ptr);
       for (int64_t i = 0; i < n; ++i) t.d[(size_t)i] = host_h2f(s[i], dtype == GP_BF16);
     } else throw GpError(GP_ERR_INVALID, "gp_load_tensor: unsupported dtype");
-    e->ws.host[key] = std::move(t);
+    if (!text) {
+      e->ws.host[key] = std::move(t);
+      return;
+    }
+    TextTower& tt = e->text;
+    if (!tt.ws || tt.packed) {   // a tensor after gp_encode_text: the next call packs the weights again
+      std::unique_ptr<WeightStore> fresh(new WeightStore(e->ws.bf16, e->ws.split));
+      if (tt.ws) fresh->host = std::move(tt.ws->host);
+      GP_CUDA(cudaSetDevice(e->cfg.device));
+      tt.plans.clear();
+      tt.ws = std::move(fresh);
+      tt.packed = false;
+    }
+    tt.ws->host[key] = std::move(t);
+  });
+}
+
+gp_status gp_encode_text(gp_engine* e, const int32_t* ids_host, int n_tokens, float* out_host, void* stream) {
+  return guarded(e, [&]() {
+    if (e->finalized) throw GpError(GP_ERR_STATE, "gp_encode_text after gp_finalize: the context is a constant of the engine");
+    GP_REQUIRE(ids_host && out_host, "gp_encode_text: bad arguments");
+    GP_REQUIRE(n_tokens >= 1 && n_tokens <= kTextMaxTokens,
+               "gp_encode_text: " + std::to_string(n_tokens) + " tokens (1 to " + std::to_string(kTextMaxTokens) + ")");
+    for (int i = 0; i < n_tokens; ++i)
+      GP_REQUIRE(ids_host[i] >= 0 && ids_host[i] < kTextVocab,
+                 "gp_encode_text: token id " + std::to_string(ids_host[i]) + " outside [0, " + std::to_string(kTextVocab) + ")");
+    TextTower& tt = e->text;
+    for (const auto& kv : text_tower_spec())
+      if (!tt.ws || !tt.ws->host.count(kv.first)) throw GpError(GP_ERR_MISSING, "gp_encode_text: missing " + kv.first);
+    GP_CUDA(cudaSetDevice(e->cfg.device));
+    TextPlan* p = tt.plan(n_tokens);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    GP_CUDA(cudaMemcpyAsync(p->ids, ids_host, (size_t)n_tokens * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    for (auto& op : p->ops) GP_CUDA(op.run(s));
+    GP_CUDA(cudaMemcpyAsync(out_host, p->out, (size_t)n_tokens * kTextDim * sizeof(float), cudaMemcpyDeviceToHost, s));
+    GP_CUDA(cudaStreamSynchronize(s));
   });
 }
 
@@ -917,6 +1069,7 @@ gp_status gp_finalize(gp_engine* e) {
     e->build(b, nullptr, 1, 64, 64);
     if (e->multistep) e->steps.init(e->ws);
     e->ws.host.clear();
+    e->text = TextTower();     // the tower's weights and arenas: gp_encode_text is done once the context is fixed
     e->finalized = true;
   });
 }

@@ -255,6 +255,10 @@ class WeightStore {
   const PackedW& unet_tail();
   const PackedW& decoder_tail1();
   int unet_in_channels();
+  // the text tower's fused [q / 8 ; k ; v] projection of self-attention `p` (bias folded the same way), and a checkpoint
+  // tensor uploaded as it is, fp32 (the embedding tables)
+  const PackedW& text_qkv_w(const std::string& p);
+  const float* f32_w(const std::string& key);
 
   void compute_temb(int timestep);
   void set_timestep(int timestep);
@@ -278,6 +282,7 @@ class WeightStore {
   std::unordered_map<std::string, XattnW> xattns;
   std::unordered_map<std::string, DirectW> directs;
   std::unordered_map<std::string, float*> v_biases;
+  std::unordered_map<std::string, float*> f32s;
   std::vector<float> temb;   // [1280] time embedding for the configured timestep
   // Per-call fix_timesteps (genpercept_pipeline.py:405-408): the timestep only enters through
   // conv1.bias + time_emb_proj(silu(emb(t))) of the 22 UNet ResNets, so changing it re-folds those biases in place
@@ -298,6 +303,15 @@ T4 resnet_block(Builder& b, WeightStore& ws, const std::string& p, const std::ve
 void cross_attention(Builder& b, WeightStore& ws, const std::string& blk, const T4& x, int heads, float eps, const T4& out);
 // out [.., 4C] = GEGLU(ff.net.0.proj(x)) of transformer block `blk` (x [.., C], the projection's GEGLU epilogue)
 void geglu_projection(Builder& b, WeightStore& ws, const std::string& blk, const T4& x, const T4& out);
+
+// SD-2.1's CLIP text tower (transformers' CLIPTextModel, SURVEY.md App. A): token + position embedding, 23 pre-LN layers
+// of causal self-attention (16 heads of 64) and an exact-erf GELU MLP, final LayerNorm.  Its weights are `text.` + the
+// CLIPTextModel state-dict keys.
+constexpr int kTextVocab = 49408, kTextDim = 1024, kTextLayers = 23, kTextHeads = 16, kTextMlp = 4096;
+// The key -> shape of every tensor the tower reads.
+const std::map<std::string, std::vector<int64_t>>& text_tower_spec();
+// last_hidden_state [n, kTextDim] (fp32, `out`) of the n <= kTextMaxTokens token ids at `ids` (device), on the arena of `b`
+void text_tower(Builder& b, WeightStore& ws, int n, const int32_t* ids, float* out);
 
 // arena.cu: the per-device activation arena shared by the plans of engines with gp_set_shared_arena on.  join / leave
 // count the engines that share it (the last leave unmaps everything and frees the reservation); add maps enough for a

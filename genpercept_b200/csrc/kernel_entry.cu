@@ -420,6 +420,27 @@ gp_status gp_resize(int dtype, const void* x, int N, int H, int W, int C, int OH
   });
 }
 
+gp_status gp_causal_attention(int dtype, const void* qkv, int n, int heads, int d, void* out, void* stream) {
+  return guarded_free([&]() {
+    GP_REQUIRE(qkv && out && n >= 1 && n <= kTextMaxTokens && heads >= 1 && d >= 1 && d <= kCausalMaxD,
+               "gp_causal_attention: bad arguments (1 <= n <= 77, 1 <= d <= 64)");
+    const bool pair = storage_layout(dtype, true, "gp_causal_attention");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    GP_CUDA(causal_attention(qkv, n, heads, d, out, dtype == GP_BF16, s, pair));
+    GP_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+gp_status gp_gelu(int dtype, const void* x, int64_t n_elems, void* y, void* stream) {
+  return guarded_free([&]() {
+    GP_REQUIRE(x && y && n_elems >= 8 && n_elems % 8 == 0 && n_elems < (1LL << 30), "gp_gelu: bad arguments (n_elems % 8 == 0)");
+    const bool pair = storage_layout(dtype, true, "gp_gelu");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    GP_CUDA(gelu16(x, y, n_elems, dtype == GP_BF16, s, pair ? (int)n_elems : 0));
+    GP_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters, double* usec,
                         double* flops) {
   return guarded_free([&]() {

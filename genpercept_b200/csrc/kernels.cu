@@ -1308,4 +1308,182 @@ cudaError_t nearest_resize(const void* in, void* out, int N, int H, int W, int O
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------ CLIP text tower
+namespace {
+constexpr int kCaWarps = 8;                                    // query rows per causal-attention CTA (one per warp)
+constexpr int kCaKeysPerLane = (kTextMaxTokens + 31) / 32;
+
+// one CTA per token: row ids[t] of the token table + row t of the position table, summed in fp32
+template <bool BF16>
+__global__ void text_embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ tok, const float* __restrict__ pos,
+                                  uint16_t* __restrict__ out, int C, int lo) {
+  const int t = blockIdx.x;
+  const float* tr = tok + (long long)__ldg(ids + t) * C;
+  const float* pr = pos + (long long)t * C;
+  for (int v = threadIdx.x; v < C / 8; v += blockDim.x) {
+    float f[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) f[e] = __ldg(tr + v * 8 + e) + __ldg(pr + v * 8 + e);
+    store8<BF16>(out + (long long)t * (lo ? 2 * C : C) + v * 8, lo, f);
+  }
+}
+
+// softmax(q k^T) v with key j kept for j <= i, per head; q carries the softmax scale.  qkv: per token [q C | k C | v C]
+// (C = heads * d; [hi 3C | lo 3C] in the pair layout), out: per token [C] ([hi C | lo C]).  Grid (heads, query blocks of
+// kCaWarps rows): the CTA stages its head's keys and values 0 .. its last query in shared memory as fp32 (hi + lo), and
+// each warp owns one query row: scores with the lanes over keys, then the output with the lanes over dims.
+template <bool BF16>
+__global__ void causal_attention_kernel(const uint16_t* __restrict__ qkv, int n, int C, int d, uint16_t* __restrict__ out,
+                                        int lo_in, int lo_out) {
+  extern __shared__ float sm[];
+  const int h = blockIdx.x;
+  const int nk = min(n, (blockIdx.y + 1) * kCaWarps);          // keys the block's last query sees
+  const int ks = d + 1;                                         // padded row: lanes reading key j hit different banks
+  float* K = sm;
+  float* V = K + nk * ks;
+  float* Q = V + nk * ks;
+  float* P = Q + kCaWarps * d;
+  const long long in_stride = lo_in ? 2LL * lo_in : 3LL * C;
+  for (int idx = threadIdx.x; idx < nk * d; idx += blockDim.x) {
+    const int j = idx / d, c = idx % d;
+    const uint16_t* row = qkv + j * in_stride + h * d + c;
+    K[j * ks + c] = load1<BF16>(row + C, lo_in);
+    V[j * ks + c] = load1<BF16>(row + 2 * C, lo_in);
+  }
+  const int w = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const int i = blockIdx.y * kCaWarps + w;
+  if (i < n)
+    for (int c = lane; c < d; c += 32) Q[w * d + c] = load1<BF16>(qkv + i * in_stride + h * d + c, lo_in);
+  __syncthreads();
+  if (i >= n) return;
+  const float* q = Q + w * d;
+  float s[kCaKeysPerLane];
+  float m = -INFINITY;
+#pragma unroll
+  for (int r = 0; r < kCaKeysPerLane; ++r) {
+    const int j = lane + 32 * r;
+    s[r] = -INFINITY;
+    if (j <= i) {
+      float acc = 0.f;
+      for (int c = 0; c < d; ++c) acc = fmaf(q[c], K[j * ks + c], acc);
+      s[r] = acc;
+      m = fmaxf(m, acc);
+    }
+  }
+  m = warp_max(m);
+  float l = 0.f;
+#pragma unroll
+  for (int r = 0; r < kCaKeysPerLane; ++r) {
+    const int j = lane + 32 * r;
+    const float p = j <= i ? expf(s[r] - m) : 0.f;
+    l += p;
+    if (j < nk) P[w * kTextMaxTokens + j] = p;
+  }
+  l = warp_sum(l);
+  __syncwarp();
+  const float inv = 1.f / l;
+  const long long out_stride = lo_out ? 2LL * lo_out : C;
+  for (int c = lane; c < d; c += 32) {
+    float acc = 0.f;
+    for (int j = 0; j <= i; ++j) acc = fmaf(P[w * kTextMaxTokens + j], V[j * ks + c], acc);
+    store1<BF16>(out + i * out_stride + h * d + c, lo_out, acc * inv);
+  }
+}
+
+// x (1 + erf(x / sqrt 2)) / 2 as x erfc(-x / sqrt 2) / 2: no cancellation where erf(x / sqrt 2) nears -1
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * erfcf(-x * 0.70710678118654752f); }
+
+template <bool BF16>
+__global__ void gelu_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, long long total_vec, int nvec, int lo) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total_vec;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long off = lo ? (i / nvec) * (2LL * lo) + (i % nvec) * 8 : i * 8;   // [pixel][hi C | lo C]
+    float a[8];
+    load8<BF16>(in + off, lo, a);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) a[e] = gelu_erf(a[e]);
+    store8<BF16>(out + off, lo, a);
+  }
+}
+
+// LayerNorm of 16-bit (or pair) rows of C <= 32 * 8 * kLnF32Vec channels into fp32 rows: one warp per token, the row in
+// registers, two-pass mean and variance
+constexpr int kLnF32Vec = 4;
+template <bool BF16>
+__global__ void layernorm_f32_kernel(const uint16_t* __restrict__ x, float* __restrict__ y, long long tokens, int C,
+                                     const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int lo) {
+  const long long t = (long long)blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+  const int lane = threadIdx.x % 32;
+  if (t >= tokens) return;
+  const uint16_t* row = x + t * (lo ? 2 * C : C);
+  const int nvec = C / 8;
+  float f[kLnF32Vec][8];
+  float sum = 0.f;
+#pragma unroll
+  for (int k = 0; k < kLnF32Vec; ++k) {
+    const int v = lane + 32 * k;
+    if (v < nvec) {
+      load8<BF16>(row + v * 8, lo, f[k]);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) sum += f[k][e];
+    }
+  }
+  const float mean = warp_sum(sum) / C;
+  float sq = 0.f;
+#pragma unroll
+  for (int k = 0; k < kLnF32Vec; ++k)
+    if (lane + 32 * k < nvec)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) sq += (f[k][e] - mean) * (f[k][e] - mean);
+  const float rstd = rsqrtf(warp_sum(sq) / C + eps);
+#pragma unroll
+  for (int k = 0; k < kLnF32Vec; ++k) {
+    const int v = lane + 32 * k;
+    if (v < nvec)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int c = v * 8 + e;
+        y[t * C + c] = (f[k][e] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c);
+      }
+  }
+}
+}  // namespace
+
+cudaError_t text_embed(const int32_t* ids, int n, const float* tok, const float* pos, void* out, int C, bool bf16,
+                       cudaStream_t s, bool split) {
+  if (n < 1 || C % 8) return cudaErrorInvalidValue;
+  GP_DISPATCH_BF16(bf16, (launch(text_embed_kernel<BF>, (unsigned)n, 128, 0, s, ids, tok, pos, reinterpret_cast<uint16_t*>(out),
+                                 C, split ? C : 0)));
+  return cudaGetLastError();
+}
+
+cudaError_t causal_attention(const void* qkv, int n, int heads, int d, void* out, bool bf16, cudaStream_t s, bool split) {
+  if (n < 1 || n > kTextMaxTokens || heads < 1 || d < 1 || d > kCausalMaxD) return cudaErrorInvalidValue;
+  const int C = heads * d;
+  const int qblocks = (n + kCaWarps - 1) / kCaWarps;
+  const size_t smem = ((size_t)2 * n * (d + 1) + (size_t)kCaWarps * d + (size_t)kCaWarps * kTextMaxTokens) * sizeof(float);
+  GP_DISPATCH_BF16(bf16, (launch(causal_attention_kernel<BF>, dim3((unsigned)heads, (unsigned)qblocks), kCaWarps * 32, smem, s,
+                                 reinterpret_cast<const uint16_t*>(qkv), n, C, d, reinterpret_cast<uint16_t*>(out),
+                                 split ? 3 * C : 0, split ? C : 0)));
+  return cudaGetLastError();
+}
+
+cudaError_t gelu16(const void* in, void* out, long long n, bool bf16, cudaStream_t s, int split_c) {
+  if (n % 8 || split_c % 8) return cudaErrorInvalidValue;
+  const long long total_vec = n / 8;        // n = pixels * C logical elements
+  GP_DISPATCH_BF16(bf16, (launch(gelu_kernel<BF>, blocks_for(total_vec, 256), 256, 0, s,
+                                 reinterpret_cast<const uint16_t*>(in), reinterpret_cast<uint16_t*>(out), total_vec,
+                                 split_c ? split_c / 8 : 1, split_c)));
+  return cudaGetLastError();
+}
+
+cudaError_t layernorm_f32(const void* x, float* y, long long tokens, int C, const float* gamma, const float* beta, float eps,
+                          bool bf16, cudaStream_t s, bool split) {
+  if (tokens < 1 || C % 8 || C / 8 > 32 * kLnF32Vec) return cudaErrorInvalidValue;
+  const int wpb = 4;
+  GP_DISPATCH_BF16(bf16, (launch(layernorm_f32_kernel<BF>, (unsigned)((tokens + wpb - 1) / wpb), wpb * 32, 0, s,
+                                 reinterpret_cast<const uint16_t*>(x), y, tokens, C, gamma, beta, eps, split ? C : 0)));
+  return cudaGetLastError();
+}
+
 }  // namespace gp

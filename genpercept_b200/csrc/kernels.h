@@ -116,6 +116,21 @@ struct BiasSegment { float* dst; int off; int len; };
 cudaError_t bias_scatter(const float* row, const BiasSegment* segs, int nseg, cudaStream_t s);
 cudaError_t latent_affine(const void* in, void* out, long long npx, float pre, const float* mat, const float* bias, bool bf16,
                           cudaStream_t s, bool split = false);
+// SD-2.1's CLIP text tower (text_tower, engine.cu), 16-bit or pair rows of tokens:
+//   text_embed: out[t] = tok[ids[t]] + pos[t] (fp32 tables [*, C], the sum in fp32, then stored)
+//   causal_attention: softmax(q k^T) v per head over keys j <= i, scores and softmax in fp32 (the scale folded into q);
+//     qkv per token [q C | k C | v C] with C = heads * d ([hi 3C | lo 3C] in the pair layout), out per token [C];
+//     n <= kTextMaxTokens, d <= kCausalMaxD
+//   gelu16: exact-erf GELU, the shape of relu16
+//   layernorm_f32: LayerNorm of 16-bit (or pair: hi + lo) rows into fp32 rows [tokens, C], C <= 1024
+constexpr int kTextMaxTokens = 77;
+constexpr int kCausalMaxD = 64;
+cudaError_t text_embed(const int32_t* ids, int n, const float* tok, const float* pos, void* out, int C, bool bf16,
+                       cudaStream_t s, bool split = false);
+cudaError_t causal_attention(const void* qkv, int n, int heads, int d, void* out, bool bf16, cudaStream_t s, bool split = false);
+cudaError_t gelu16(const void* in, void* out, long long n, bool bf16, cudaStream_t s, int split_c = 0);
+cudaError_t layernorm_f32(const void* x, float* y, long long tokens, int C, const float* gamma, const float* beta, float eps,
+                          bool bf16, cudaStream_t s, bool split = false);
 // per-image (x - min) / (max - min) over HW fp32 values, in place; scratch: 2 uint32 per image.
 // dmin: lower clamp of (max - min) (0 for the DPT readout, 1e-6 in ensemble_depth); zero_min: normalise by max only
 cudaError_t minmax_normalize(float* x, int N, long long HW, unsigned int* scratch, cudaStream_t s, float dmin = 0.f, bool zero_min = false);

@@ -522,6 +522,54 @@ int WeightStore::unet_in_channels() {
   return (int)wci.shape[1];
 }
 
+// ------------------------------------------------------------------ CLIP text tower
+const std::map<std::string, std::vector<int64_t>>& text_tower_spec() {
+  static const std::map<std::string, std::vector<int64_t>> spec = [] {
+    std::map<std::string, std::vector<int64_t>> s;
+    const std::string m = "text.text_model.";
+    const int64_t D = kTextDim, F = kTextMlp;
+    s[m + "embeddings.token_embedding.weight"] = {kTextVocab, D};
+    s[m + "embeddings.position_embedding.weight"] = {kTextMaxTokens, D};
+    auto lin = [&](const std::string& k, int64_t out, int64_t in) { s[k + ".weight"] = {out, in}; s[k + ".bias"] = {out}; };
+    auto norm = [&](const std::string& k) { s[k + ".weight"] = {D}; s[k + ".bias"] = {D}; };
+    for (int i = 0; i < kTextLayers; ++i) {
+      const std::string p = m + "encoder.layers." + std::to_string(i);
+      for (const char* n : {"q_proj", "k_proj", "v_proj", "out_proj"}) lin(p + ".self_attn." + n, D, D);
+      norm(p + ".layer_norm1");
+      norm(p + ".layer_norm2");
+      lin(p + ".mlp.fc1", F, D);
+      lin(p + ".mlp.fc2", D, F);
+    }
+    norm(m + "final_layer_norm");
+    return s;
+  }();
+  return spec;
+}
+
+// [q_proj / 8 ; k_proj ; v_proj] with the biases likewise: one token GEMM writes q | k | v, the softmax scale d^-1/2 = 1/8
+// folded into the q rows (a power of two: the fold is exact)
+const PackedW& WeightStore::text_qkv_w(const std::string& p) {
+  auto it = packed.find(p + ".qkv");
+  if (it != packed.end()) return it->second;
+  const size_t DD = (size_t)kTextDim * kTextDim;
+  const float scale = 1.0f / std::sqrt((float)(kTextDim / kTextHeads));
+  std::vector<float> m(3 * DD), bias(3 * kTextDim);
+  const char* parts[3] = {".q_proj", ".k_proj", ".v_proj"};
+  for (int k = 0; k < 3; ++k) {
+    const float f = k == 0 ? scale : 1.0f;
+    const HostT &w = T(p + parts[k] + ".weight"), &b = T(p + parts[k] + ".bias");
+    for (size_t i = 0; i < DD; ++i) m[k * DD + i] = w.d[i] * f;
+    for (int i = 0; i < kTextDim; ++i) bias[k * kTextDim + i] = b.d[i] * f;
+  }
+  return mat_w(p + ".qkv", 3 * kTextDim, kTextDim, m.data(), bias);
+}
+
+const float* WeightStore::f32_w(const std::string& key) {
+  auto it = f32s.find(key);
+  if (it != f32s.end()) return it->second;
+  return f32s.emplace(key, upload(T(key).d)).first->second;
+}
+
 // ------------------------------------------------------------------ timestep
 void WeightStore::compute_temb(int timestep) {
   if (!temb.empty()) return;

@@ -46,6 +46,7 @@ def lib():
     L.gp_last_error.restype = c_char_p
     L.gp_load_tensor.argtypes = [c_void_p, c_char_p, c_void_p, c_int, POINTER(c_int64), c_int]
     L.gp_set_text_embed.argtypes = [c_void_p, c_void_p, c_int, c_int]
+    L.gp_encode_text.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p]
     L.gp_finalize.argtypes = [c_void_p]
     L.gp_plan.argtypes = [c_void_p, c_int, c_int, c_int]
     L.gp_infer.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]
@@ -93,6 +94,8 @@ def lib():
     L.gp_resnet.argtypes = [c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float] + [c_void_p] * 10 + \
         [c_void_p, c_void_p]
     L.gp_resize.argtypes = [c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    L.gp_causal_attention.argtypes = [c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
+    L.gp_gelu.argtypes = [c_int, c_void_p, c_int64, c_void_p, c_void_p]
     L.gp_bench_conv.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_double),
                                 POINTER(c_double)]
     L.gp_bench_attention.argtypes = [c_int, c_int, c_int, c_int, c_int, POINTER(c_double), POINTER(c_double)]
@@ -202,7 +205,8 @@ class Engine:
             raise RuntimeError(f"{what}: {_STATUS.get(st, st)}: {msg}")
 
     def load_state(self, component, sd):
-        """component in {unet, vae, dpt}; sd: {diffusers key: tensor}."""
+        """component in {unet, vae, dpt}: sd = {diffusers key: tensor}; or "text": sd = transformers' CLIPTextModel
+        state dict (SD-2.1's tower; checked against its shapes, the position_ids buffer ignored)."""
         for k, v in sd.items():
             t = v.detach().to("cpu")
             if t.dtype not in (torch.float32, torch.float16, torch.bfloat16):
@@ -215,6 +219,19 @@ class Engine:
     def set_text_embed(self, embed):
         e = torch.as_tensor(embed).detach().float().cpu().reshape(-1, 1024).contiguous()
         self._ck(self.L.gp_set_text_embed(self.h, c_void_p(e.data_ptr()), e.shape[0], 1024), "gp_set_text_embed")
+
+    def encode_text(self, ids):
+        """SD-2.1's CLIP text tower on the engine, in its mode (gp_encode_text): token ids (1 to 77 of them, a sequence or a
+        [1, n] / [n] tensor) -> last_hidden_state, fp32 [1, n, 1024] on the host.  Needs the "text" weights
+        (``load_state("text", ...)``) and runs only before ``finalize``, which frees the tower."""
+        ids = torch.as_tensor(ids).reshape(-1)
+        assert ids.dtype in (torch.int32, torch.int64), "token ids must be integers"
+        n = ids.numel()
+        a = np.ascontiguousarray(ids.cpu().numpy(), dtype=np.int32)
+        out = np.empty((n, 1024), dtype=np.float32)
+        self._ck(self.L.gp_encode_text(self.h, a.ctypes.data_as(c_void_p), n, out.ctypes.data_as(c_void_p), self._sp()),
+                 "gp_encode_text")
+        return torch.from_numpy(out)[None]
 
     def finalize(self):
         self._ck(self.L.gp_finalize(self.h), "gp_finalize")
@@ -629,6 +646,31 @@ def resize(x_nhwc, out_h, out_w, mode):
                          _stream_ptr(x_nhwc.device))
     _check_free(st, "gp_resize")
     return _result(y, dt)
+
+
+def causal_attention(qkv, heads):
+    """The text tower's causal self-attention through gp_causal_attention: qkv cuda [n, 3C] = per token [q | k | v] with the
+    softmax scale already in q (f16/bf16, or fp32: the pair layout, float64 result).  Returns [n, C]: softmax(q k^T) v per
+    head over keys j <= i."""
+    dt = _layout(qkv)
+    n, C3 = qkv.shape
+    C = C3 // 3
+    xa = _arg(qkv, dt)
+    y = _out((n, C), dt, qkv.device)
+    st = lib().gp_causal_attention(dt, _ptr(xa), n, heads, C // heads, _ptr(y), _stream_ptr(qkv.device))
+    _check_free(st, "gp_causal_attention")
+    return _result(y, dt)
+
+
+def gelu(x):
+    """Exact-erf GELU through gp_gelu on cuda x of any shape (f16/bf16, or fp32: the pair layout over the whole tensor,
+    float64 result); x.numel() % 8 == 0."""
+    dt = _layout(x)
+    flat = x.reshape(1, -1)
+    xa = _arg(flat, dt)
+    y = _out(tuple(flat.shape), dt, x.device)
+    _check_free(lib().gp_gelu(dt, _ptr(xa), flat.numel(), _ptr(y), _stream_ptr(x.device)), "gp_gelu")
+    return _result(y, dt).reshape(x.shape)
 
 
 RESIZE_MODES = {"bilinear": 0, "bicubic": 1}

@@ -41,6 +41,21 @@ def _checkpoint_scheduler(root, kw):
     kw["scheduler"] = path
 
 
+def _checkpoint_text_tower(root, kw):
+    """The SD-2.1 folder's text tower when no text_embed / text_encoder is passed: ``<root>/text_encoder/`` as a path,
+    which the pipeline reads as a state dict (model.safetensors or .bin, honouring `variant`) for the engine's own tower,
+    and transformers' CLIPTokenizer from ``<root>/tokenizer`` unless a tokenizer is passed.  No CLIPTextModel is built."""
+    if kw.get("text_embed") is not None or kw.get("text_encoder") is not None:
+        return
+    folder = os.path.join(root, "text_encoder")
+    if not os.path.isdir(folder):
+        return
+    kw["text_encoder"] = folder
+    if kw.get("tokenizer") is None:
+        from transformers import CLIPTokenizer
+        kw["tokenizer"] = CLIPTokenizer.from_pretrained(os.path.join(root, "tokenizer"))
+
+
 @dataclass
 class GenPerceptOutput:
     """pred_np: result in [0,1]; pred_colored: PIL image or None (genpercept_pipeline.py:50-62)."""
@@ -154,6 +169,10 @@ class GenPerceptPipeline:
             self._engine.load_state("dpt", _as_state_dict(customized_head))
         self._engine.load_state("unet", unet_sd)
         self._engine.load_state("vae", vae_sd)
+        # the text tower's weights only (a module's forward never runs): encode_text runs SD-2.1's CLIP tower on the
+        # engine, in its mode
+        if text_encoder is not None and text_embed is None:
+            self._engine.load_state("text", _as_state_dict(text_encoder, variant))
         self._finalized = False
         if text_embed is not None:
             self._set_text_embed(text_embed)
@@ -171,10 +190,7 @@ class GenPerceptPipeline:
             kw["vae"] = os.path.join(root, "vae")
         if kw.get("unet") is None:
             kw["unet"] = os.path.join(root, "unet")
-        if kw.get("text_embed") is None and kw.get("text_encoder") is None and os.path.isdir(os.path.join(root, "text_encoder")):
-            from transformers import CLIPTextModel, CLIPTokenizer
-            kw["text_encoder"] = CLIPTextModel.from_pretrained(os.path.join(root, "text_encoder"))
-            kw["tokenizer"] = CLIPTokenizer.from_pretrained(os.path.join(root, "tokenizer"))
+        _checkpoint_text_tower(root, kw)
         return cls(torch_dtype=torch_dtype, variant=variant, **kw)
 
     @classmethod
@@ -186,11 +202,7 @@ class GenPerceptPipeline:
         from . import loader
         _checkpoint_scheduler(checkpoint, kw)
         parts = loader.assemble(checkpoint, unet=unet, lora_rank=lora_rank, variant=kw.get("variant"))
-        root = str(checkpoint)
-        if kw.get("text_embed") is None and kw.get("text_encoder") is None and os.path.isdir(os.path.join(root, "text_encoder")):
-            from transformers import CLIPTextModel, CLIPTokenizer
-            kw["text_encoder"] = CLIPTextModel.from_pretrained(os.path.join(root, "text_encoder"))
-            kw["tokenizer"] = CLIPTokenizer.from_pretrained(os.path.join(root, "tokenizer"))
+        _checkpoint_text_tower(str(checkpoint), kw)
         return cls(unet=parts["unet"], vae=parts["vae"], customized_head=parts["customized_head"], **kw)
 
     def to(self, *a, **k):
@@ -228,14 +240,14 @@ class GenPerceptPipeline:
         self._engine.set_text_embed(e)
 
     def encode_text(self, prompt):
-        """genpercept_pipeline.py:360-372: tokenizer(prompt, padding='do_not_pad') -> CLIP -> [1,2,1024]."""
+        """genpercept_pipeline.py:360-372: tokenizer(prompt, padding='do_not_pad') on the host, then SD-2.1's CLIP text
+        tower on the engine (gp_encode_text, in the engine's mode) -> [1, n, 1024]; the empty prompt gives n = 2."""
         if self.text_encoder is None or self.tokenizer is None:
             raise RuntimeError("no text_encoder/tokenizer given: pass text_embed= (e.g. the fixture "
                                "tests/golden/empty_text_embed_2x1024.npy)")
         ti = self.tokenizer(prompt, padding="do_not_pad", max_length=self.tokenizer.model_max_length,
                             truncation=True, return_tensors="pt")
-        with torch.no_grad():
-            self._set_text_embed(self.text_encoder(ti.input_ids)[0])
+        self._set_text_embed(self._engine.encode_text(ti.input_ids))
 
     def _ensure_ready(self, prompt=""):
         if self.text_embed is None:

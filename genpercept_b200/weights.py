@@ -228,5 +228,40 @@ def synth_text_embed(seed=1234, n_tokens=2):
     return torch.randn((1, n_tokens, 1024), generator=gen, dtype=torch.float32)
 
 
+TEXT_VOCAB, TEXT_POSITIONS, TEXT_DIM, TEXT_LAYERS, TEXT_MLP = 49408, 77, 1024, 23, 4096
+
+
+def text_spec():
+    """SD-2.1's CLIP text tower (transformers' CLIPTextModel, SURVEY.md App. A) under its own state-dict keys."""
+    s = OrderedDict()
+    m = "text_model."
+    s[m + "embeddings.token_embedding.weight"] = ((TEXT_VOCAB, TEXT_DIM), "embedding")
+    s[m + "embeddings.position_embedding.weight"] = ((TEXT_POSITIONS, TEXT_DIM), "embedding")
+    for i in range(TEXT_LAYERS):
+        p = f"{m}encoder.layers.{i}."
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            _lin(s, p + "self_attn." + n, TEXT_DIM, TEXT_DIM)
+        _norm(s, p + "layer_norm1", TEXT_DIM)
+        _lin(s, p + "mlp.fc1", TEXT_DIM, TEXT_MLP)
+        _lin(s, p + "mlp.fc2", TEXT_MLP, TEXT_DIM)
+        _norm(s, p + "layer_norm2", TEXT_DIM)
+    _norm(s, m + "final_layer_norm", TEXT_DIM)
+    return s
+
+
+def synth_text_state(seed=1234):
+    """Seeded synthetic fp32 weights of SD-2.1's CLIP text tower (``text_spec``), from a generator of their own, so no
+    other fixture's stream moves.  Embedding rows have std 0.5, so token and position both matter after the first
+    LayerNorm; the linear layers keep O(1) activations as in ``synth_state``."""
+    sd = OrderedDict()
+    gen = torch.Generator().manual_seed(seed + 4242)
+    for k, (shape, kind) in text_spec().items():
+        if kind == "embedding":
+            sd[k] = torch.randn(shape, generator=gen, dtype=torch.float32) * 0.5
+        else:
+            sd.update(_synth(OrderedDict([(k, (shape, kind))]), gen))
+    return sd
+
+
 def param_count(spec):
     return sum(int(np.prod(s)) for s, _ in spec.values())

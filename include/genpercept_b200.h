@@ -62,7 +62,7 @@ void gp_destroy(gp_engine* e);
 const char* gp_last_error(gp_engine* e);
 
 /* replaces: load_state_dict of the diffusers-format checkpoints (run.py:336-357, :296-312).
- * `key` = "<component>.<diffusers key>", component in {unet, vae, dpt}.  Host pointer, copied. */
+ * `key` = "<component>.<diffusers key>", component in {unet, vae, dpt}, or "text" (gp_encode_text).  Host pointer, copied. */
 gp_status gp_load_tensor(gp_engine* e, const char* key, const void* host_ptr, int dtype,
                          const int64_t* shape, int ndim);
 /* replaces: encode_text()'s cached self.text_embed (genpercept_pipeline.py:360-372, :425-429).
@@ -70,7 +70,18 @@ gp_status gp_load_tensor(gp_engine* e, const char* key, const void* host_ptr, in
  * length the general one (context projections folded into two 1x1 GEMMs around a per-head softmax).  The
  * context is a constant of the engine from gp_finalize on, like the reference's cached self.text_embed. */
 gp_status gp_set_text_embed(gp_engine* e, const float* host_ptr, int n_tokens, int dim);
-/* folds constants (SURVEY.md App. C), re-packs weights K-major 16-bit, uploads. */
+/* replaces: encode_text()'s text_encoder(text_input_ids)[0] (genpercept_pipeline.py:360-372), SD-2.1's CLIPTextModel, on
+ * the engine in its mode (16-bit, or the high-precision pair layout).  ids_host: n_tokens token ids (int32, host) as the
+ * tokenizer gives them, 1 <= n_tokens <= 77, each in [0, 49408); out_host: fp32 [n_tokens, 1024] = last_hidden_state after
+ * final_layer_norm, ready for gp_set_text_embed.  Its weights are gp_load_tensor's component "text": "text." + the
+ * CLIPTextModel state-dict keys ("text.text_model.encoder.layers.0.self_attn.q_proj.weight", ...; the position_ids buffer
+ * is ignored), each checked against SD-2.1's shapes on load (GP_ERR_INVALID otherwise, e.g. SD-1.x's d = 768 tower).  The
+ * tower packs its own weights and an arena per n_tokens on first use, apart from the image plans (gp_plan_info's weight
+ * bytes do not count them), and runs on `stream`; it returns after the copy.  Errors leave the engine usable: a bad id or
+ * n_tokens GP_ERR_INVALID, a text tensor never loaded GP_ERR_MISSING, a call after gp_finalize GP_ERR_STATE. */
+gp_status gp_encode_text(gp_engine* e, const int32_t* ids_host, int n_tokens, float* out_host, void* stream);
+/* folds constants (SURVEY.md App. C), re-packs weights K-major 16-bit, uploads.  Frees the text tower's host tensors,
+ * device weights and arenas: from here on the context is a constant of the engine. */
 gp_status gp_finalize(gp_engine* e);
 
 /* builds the static op list, activation arena and (optionally) CUDA graph for one input shape.  Any H, W >= 32: the
@@ -270,6 +281,13 @@ gp_status gp_resnet(int dtype, const void* x, int Cx, const void* skip, int Cski
 /* F.interpolate(x [N,H,W,C], size=(OH,OW)) -> y [N,OH,OW,C]: mode 0 nearest (the UNet's Upsample2D to a skip's size),
  * 1 bilinear with align_corners=False (the DPT fusion stage's resize of a skip feature).  C % 8 == 0. */
 gp_status gp_resize(int dtype, const void* x, int N, int H, int W, int C, int OH, int OW, int mode, void* y, void* stream);
+/* The text tower's kernels (gp_encode_text), each on caller buffers, synchronised; dtype GP_F16, GP_BF16 or GP_F16_PAIR.
+ * gp_causal_attention: out [n, C] = softmax(q k^T) v per head over keys j <= i (scores and softmax in fp32), C = heads * d,
+ * from qkv [n, 3C] = per token [q | k | v] (the fused projection's output, the softmax scale already in q); pair layout:
+ * per token [hi 3C | lo 3C] in, [hi C | lo C] out.  1 <= n <= 77, 1 <= d <= 64.
+ * gp_gelu: y = x * (1 + erf(x / sqrt 2)) / 2 over n_elems values (n_elems % 8 == 0); pair layout: [hi n_elems | lo n_elems]. */
+gp_status gp_causal_attention(int dtype, const void* qkv, int n, int heads, int d, void* out, void* stream);
+gp_status gp_gelu(int dtype, const void* x, int64_t n_elems, void* y, void* stream);
 /* ---- pre/post-processing around the hot path (SURVEY.md §8 f1); buffers may be host or device ------------
  * gp_resize_aa replaces torchvision.transforms.functional.resize(tensor, size, interpolation, antialias=True)
  * as called by resize_max_res (/root/reference/genpercept/util/image_util.py:75-105) and by the resize back
