@@ -5,7 +5,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["igemm.cu", "igemm_patch.cu", "fattn.cu", "fattn512.cu", "kernels.cu", "imgproc.cu", "evaluate.cu", "builder.cu", "weights.cu", "arena.cu", "engine.cu",
+SOURCES = ["igemm.cu", "igemm_patch.cu", "fattn.cu", "fattn512.cu", "kernels.cu", "imgproc.cu", "jpeg.cu", "evaluate.cu", "builder.cu", "weights.cu", "arena.cu", "engine.cu",
            "kernel_entry.cu"]
 LIB = os.path.join(HERE, "libgenpercept_b200.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

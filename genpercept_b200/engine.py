@@ -107,6 +107,10 @@ def lib():
                               c_void_p]
     L.gp_quantize.argtypes = [c_void_p, c_int, c_size_t, c_int, c_void_p, c_int, c_void_p]
     L.gp_resize_pil.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p]
+    L.gp_jpeg_probe.argtypes = [c_char_p, c_size_t, POINTER(c_int), POINTER(c_int), POINTER(c_int64)]
+    L.gp_jpeg_decode.argtypes = [c_char_p, c_size_t, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p]
+    L.gp_jpeg_last_error.argtypes = []
+    L.gp_jpeg_last_error.restype = c_char_p
     L.gp_v1_postprocess.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p]
     L.gp_depth_align.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
@@ -747,6 +751,43 @@ def resize_pil(img_hwc, out_h, out_w, device=None):
                              _stream_ptr())
     _check_free(st, "gp_resize_pil")
     return y
+
+
+def jpeg_probe(data):
+    """Host-only check of a JPEG file's bytes (gp_jpeg_probe): (H, W, workspace_bytes) when ``decode_jpeg`` takes the
+    stream; ``ValueError`` with the reason otherwise."""
+    data = bytes(data)
+    H, W, ws = c_int(), c_int(), c_int64()
+    if lib().gp_jpeg_probe(data, len(data), byref(H), byref(W), byref(ws)) != 0:
+        raise ValueError(f"JPEG not taken by the GPU decoder: {lib().gp_jpeg_last_error().decode()}")
+    return H.value, W.value, ws.value
+
+
+def decode_jpeg(data, device=None, layout="chw"):
+    """``np.asarray(Image.open(f).convert("RGB"))`` of a JPEG file's bytes, byte for byte, decoded on the GPU
+    (gp_jpeg_decode).  Returns uint8 [3,H,W] (``layout="chw"``) or [H,W,3] (``"hwc"``) on `device` (default: the
+    current cuda device).  Raises ``ValueError`` for a stream the decoder does not take, a corrupt one, or one whose
+    parallel Huffman decode did not converge.  The workspace comes from torch's caching allocator."""
+    assert layout in ("chw", "hwc")
+    data = bytes(data)
+    H, W, ws_bytes = jpeg_probe(data)
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(dev):
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        if layout == "chw":
+            out = torch.empty((3, H, W), dtype=torch.uint8, device=dev)
+            strides = (W, 1, H * W)
+        else:
+            out = torch.empty((H, W, 3), dtype=torch.uint8, device=dev)
+            strides = (W * 3, 3, 1)
+        st = lib().gp_jpeg_decode(data, len(data), c_void_p(ws.data_ptr()), ws_bytes, c_void_p(out.data_ptr()),
+                                  *strides, _stream_ptr(dev))
+    if st == 1:
+        raise ValueError(f"GPU JPEG decode failed: {lib().gp_jpeg_last_error().decode()}")
+    _check_free(st, "gp_jpeg_decode")
+    return out
 
 
 V1_TASKS = {"depth": 0, "normal": 1, "seg": 2, "sr": 2}

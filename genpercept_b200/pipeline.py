@@ -23,7 +23,7 @@ from torchvision.transforms.functional import pil_to_tensor, resize
 from . import engine as E
 from . import weights as W
 from .engine import Engine
-from .image_util import _lut, get_tv_resample_method, resize_max_res
+from .image_util import _lut, decode_unloaded_jpeg, get_tv_resample_method, resize_max_res
 
 ONE_CHANNEL_MODES = ("depth", "matting", "dis", "disparity")     # genpercept_pipeline.py:523
 _NO_SCHEDULER = "the multi-step archs need a scheduler (hf_configs/scheduler_beta_*/scheduler_config.json)"
@@ -360,7 +360,10 @@ def preprocess(input_image, processing_res, resample_method, device):
     on `device` in [-1,1]."""
     resample = get_tv_resample_method(resample_method)
     if isinstance(input_image, Image.Image):
-        rgb = pil_to_tensor(input_image.convert("RGB")).unsqueeze(0)
+        rgb = None
+        if processing_res <= 0 or resample_method in E.RESIZE_MODES:   # the nearest modes resize on the host
+            rgb = decode_unloaded_jpeg(input_image, device, "chw")      # None: Pillow decodes, as the reference does
+        rgb = (pil_to_tensor(input_image.convert("RGB")) if rgb is None else rgb).unsqueeze(0)
     elif isinstance(input_image, torch.Tensor):
         rgb = input_image
     else:

@@ -26,7 +26,7 @@ from PIL import Image
 from . import engine as E
 from . import weights as W
 from .engine import Engine
-from .image_util import _lut
+from .image_util import _lut, decode_unloaded_jpeg
 from .pipeline import GenPerceptOutput, _as_state_dict
 
 __all__ = ["GenPerceptPipeline", "GenPerceptOutput"]
@@ -133,7 +133,8 @@ class GenPerceptPipeline:
             if size != (w, h):
                 img = img.resize(size)
             img = img.convert("RGB")
-        return E.resize_pil(np.asarray(img), size[1], size[0], device=self.device)[None]
+        hwc = decode_unloaded_jpeg(img, self.device, "hwc")             # None: Pillow decodes
+        return E.resize_pil(np.asarray(img) if hwc is None else hwc, size[1], size[0], device=self.device)[None]
 
     # ------------------------------------------------------------------ the v1 call
     @torch.no_grad()
