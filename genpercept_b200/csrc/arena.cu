@@ -218,9 +218,10 @@ void shared_arena_wait(int device, cudaStream_t s) {
   GP_CUDA(cudaStreamWaitEvent(s, pool(device).last_use, 0));
 }
 
-void shared_arena_record(int device, cudaStream_t s) {
+void shared_arena_record(int device, cudaStream_t s) noexcept {
   std::lock_guard<std::mutex> lk(g_mu);
-  GP_CUDA(cudaEventRecord(pool(device).last_use, s));
+  auto it = g_pools.find(device);
+  if (it != g_pools.end()) cudaEventRecord(it->second.last_use, s);
 }
 
 }  // namespace gp
@@ -238,16 +239,15 @@ gp_status gp_shared_arena_info(int device, int64_t* mapped_bytes, int64_t* reser
 }
 
 gp_status gp_shared_arena_fill(int device, int byte, void* stream) {
-  std::lock_guard<std::mutex> lk(gp::g_mu);
-  auto it = gp::g_pools.find(device);
-  if (it == gp::g_pools.end()) return GP_ERR_STATE;
-  gp::Pool& p = it->second;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (cudaSetDevice(device) != cudaSuccess || cudaStreamWaitEvent(s, p.last_use, 0) != cudaSuccess ||
-      (p.mapped && cudaMemsetAsync(reinterpret_cast<void*>(p.base), byte & 0xFF, p.mapped, s) != cudaSuccess) ||
-      cudaEventRecord(p.last_use, s) != cudaSuccess)
-    return GP_ERR_CUDA;
-  return GP_OK;
+  return gp::guarded_call([&]() {
+    std::lock_guard<std::mutex> lk(gp::g_mu);
+    gp::Pool& p = gp::pool(device);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    GP_CUDA(cudaSetDevice(device));
+    GP_CUDA(cudaStreamWaitEvent(s, p.last_use, 0));
+    if (p.mapped) GP_CUDA(cudaMemsetAsync(reinterpret_cast<void*>(p.base), byte & 0xFF, p.mapped, s));
+    GP_CUDA(cudaEventRecord(p.last_use, s));
+  });
 }
 
 }  // extern "C"

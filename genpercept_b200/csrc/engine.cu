@@ -205,10 +205,7 @@ struct ArenaUse {
   const Plan* p;
   cudaStream_t s;
   ArenaUse(const Plan* plan, cudaStream_t st) : p(plan), s(st) { if (p->shared) shared_arena_wait(p->device, s); }
-  ~ArenaUse() {
-    if (!p->shared) return;
-    try { shared_arena_record(p->device, s); } catch (const GpError&) {}   // the call already reports the CUDA error
-  }
+  ~ArenaUse() { if (p->shared) shared_arena_record(p->device, s); }
 };
 
 // The UNet's 22 time-embedded ResNets (the conv1 biases a timestep changes) in the order of a step's bias row: down
@@ -789,17 +786,9 @@ template <class F>
 gp_status guarded(gp_engine* e, F f) {
   if (!e) return GP_ERR_INVALID;
   if (e->poisoned) { e->err = "engine poisoned by an earlier CUDA error: " + e->err; return GP_ERR_CUDA; }
-  try {
-    f();
-    return GP_OK;
-  } catch (const GpError& ex) {
-    e->err = ex.what();
-    if (ex.st == GP_ERR_CUDA) e->poisoned = true;
-    return ex.st;
-  } catch (const std::exception& ex) {
-    e->err = ex.what();
-    return GP_ERR_INVALID;
-  }
+  const gp_status st = run_guarded(f, e->err);
+  if (st == GP_ERR_CUDA) e->poisoned = true;
+  return st;
 }
 
 cudaError_t run_ops(Plan* p, int stage_lo, int stage_hi, int out_channels, cudaStream_t s) {
@@ -964,29 +953,38 @@ const T4& named_tensor(const Plan* p, const char* name, int* creal) {
 extern "C" {
 
 gp_status gp_create(const gp_config* cfg, gp_engine** out) {
-  if (!cfg || !out) return GP_ERR_INVALID;
-  *out = nullptr;
-  if (cfg->dtype != GP_F16 && cfg->dtype != GP_BF16) return GP_ERR_INVALID;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= cfg->device) return GP_ERR_CUDA;
-  if (cudaSetDevice(cfg->device) != cudaSuccess) return GP_ERR_CUDA;
-  cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 9) return GP_ERR_CUDA;   // sm_90a only
-  gp_engine* e = new gp_engine();
-  e->cfg = *cfg;
-  if (e->cfg.timestep <= 0) e->cfg.timestep = 1;
-  e->ws.bf16 = cfg->dtype == GP_BF16;
-  e->ws.split = cfg->precision == 1;
-  e->multistep = cfg->arch == 1;
-  if (cfg->arch != 0 && cfg->arch != 1) { delete e; return GP_ERR_INVALID; }
-  if (cfg->precision != 0 && cfg->precision != 1) { delete e; return GP_ERR_INVALID; }
-  *out = e;
-  return GP_OK;
+  return guarded_call([&]() {
+    GP_REQUIRE(cfg && out, "gp_create: null config or output pointer");
+    *out = nullptr;
+    GP_REQUIRE(cfg->dtype == GP_F16 || cfg->dtype == GP_BF16, "gp_create: dtype must be GP_F16 or GP_BF16");
+    int ndev = 0;
+    GP_CUDA(cudaGetDeviceCount(&ndev));
+    const std::string dev = std::to_string(cfg->device);
+    if (ndev <= cfg->device)
+      throw GpError(GP_ERR_CUDA, "gp_create: no CUDA device " + dev + " (" + std::to_string(ndev) + " visible)");
+    GP_CUDA(cudaSetDevice(cfg->device));
+    cudaDeviceProp prop;
+    GP_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
+    if (prop.major != 9)
+      throw GpError(GP_ERR_CUDA, "gp_create: device " + dev + " is sm_" + std::to_string(prop.major * 10 + prop.minor) +
+                                     "; this library runs on sm_90a only");
+    GP_REQUIRE(cfg->arch == 0 || cfg->arch == 1, "gp_create: arch must be 0 (one-step) or 1 (multi-step)");
+    GP_REQUIRE(cfg->precision == 0 || cfg->precision == 1, "gp_create: precision must be 0 (default) or 1 (high)");
+    gp_engine* e = new gp_engine();   // nothing below throws
+    e->cfg = *cfg;
+    if (e->cfg.timestep <= 0) e->cfg.timestep = 1;
+    e->ws.bf16 = cfg->dtype == GP_BF16;
+    e->ws.split = cfg->precision == 1;
+    e->multistep = cfg->arch == 1;
+    *out = e;
+  });
 }
 
 void gp_destroy(gp_engine* e) { delete e; }
 
 const char* gp_last_error(gp_engine* e) { return e ? e->err.c_str() : "null engine"; }
+
+const char* gp_last_call_error(void) { return call_error().c_str(); }
 
 gp_status gp_load_tensor(gp_engine* e, const char* key, const void* host_ptr, int dtype, const int64_t* shape, int ndim) {
   return guarded(e, [&]() {
@@ -1169,31 +1167,42 @@ gp_status gp_set_shared_arena(gp_engine* e, int enable) {
 }
 
 gp_status gp_tile_shape(int cout, int cin, int ks, int images, int h, int w, int tokens_mode, int num_sms, int* bn, int* mt) {
-  if (!bn || !mt || cout < 1 || cin < 1 || ks < 1 || images < 1 || h < 1 || w < 1 || num_sms < 1) return GP_ERR_INVALID;
-  gp::tile_shape_for(cout, (double)cin * ks * ks, tokens_mode != 0, images, w, h, num_sms, bn, mt);
-  return GP_OK;
+  return guarded_call([&]() {
+    GP_REQUIRE(bn && mt, "gp_tile_shape: null output pointer");
+    GP_REQUIRE(cout >= 1 && cin >= 1 && ks >= 1 && images >= 1 && h >= 1 && w >= 1 && num_sms >= 1,
+               "gp_tile_shape: every size must be at least 1");
+    gp::tile_shape_for(cout, (double)cin * ks * ks, tokens_mode != 0, images, w, h, num_sms, bn, mt);
+  });
 }
 
 gp_status gp_conv_tile(int cin, int csc, int cout, int images, int h, int w, int num_sms, int* bn, int* mt, int* patch) {
-  if (!bn || !mt || !patch || cin < 1 || csc < 0 || cout < 1 || images < 1 || h < 1 || w < 1 || num_sms < 1) return GP_ERR_INVALID;
-  gp::tile_shape_for(cout, (double)cin * 9 + csc, false, images, w, h, num_sms, bn, mt);
-  const bool staged = cout % 64 == 0 && *bn % 64 == 0;   // Builder::conv: the staged epilogue of a 16-bit NHWC output
-  *patch = staged && gp::patch_tile_fits(images, h, w, cin, csc, cout, *bn, *mt, num_sms) ? 1 : 0;
-  return GP_OK;
+  return guarded_call([&]() {
+    GP_REQUIRE(bn && mt && patch, "gp_conv_tile: null output pointer");
+    GP_REQUIRE(cin >= 1 && csc >= 0 && cout >= 1 && images >= 1 && h >= 1 && w >= 1 && num_sms >= 1,
+               "gp_conv_tile: every size must be at least 1 (csc at least 0)");
+    gp::tile_shape_for(cout, (double)cin * 9 + csc, false, images, w, h, num_sms, bn, mt);
+    const bool staged = cout % 64 == 0 && *bn % 64 == 0;   // Builder::conv: the staged epilogue of a 16-bit NHWC output
+    *patch = staged && gp::patch_tile_fits(images, h, w, cin, csc, cout, *bn, *mt, num_sms) ? 1 : 0;
+  });
 }
 
 gp_status gp_step_bias_layout(int capacity, int* n_segments, int* offsets, int* lengths) {
-  if (!n_segments) return GP_ERR_INVALID;
-  const auto layout = step_bias_layout();
-  *n_segments = (int)layout.size();
-  if (capacity < (int)layout.size()) return (offsets || lengths) ? GP_ERR_INVALID : GP_OK;
-  int off = 0;
-  for (size_t k = 0; k < layout.size(); ++k) {
-    if (offsets) offsets[k] = off;
-    if (lengths) lengths[k] = layout[k].second;
-    off += layout[k].second;
-  }
-  return GP_OK;
+  return guarded_call([&]() {
+    GP_REQUIRE(n_segments, "gp_step_bias_layout: null n_segments");
+    const auto layout = step_bias_layout();
+    *n_segments = (int)layout.size();
+    if (capacity < (int)layout.size()) {
+      GP_REQUIRE(!offsets && !lengths, "gp_step_bias_layout: capacity " + std::to_string(capacity) + " is below the " +
+                                           std::to_string(layout.size()) + " segments");
+      return;
+    }
+    int off = 0;
+    for (size_t k = 0; k < layout.size(); ++k) {
+      if (offsets) offsets[k] = off;
+      if (lengths) lengths[k] = layout[k].second;
+      off += layout[k].second;
+    }
+  });
 }
 
 gp_status gp_set_timestep(gp_engine* e, int timestep) {

@@ -7,7 +7,6 @@
 #include <algorithm>
 #include <functional>
 #include <map>
-#include <stdexcept>
 #include <string>
 #include <unordered_map>
 #include <utility>
@@ -16,23 +15,9 @@
 #include "../../include/genpercept_b200.h"
 #include "igemm.h"
 #include "kernels.h"
+#include "status.h"
 
 namespace gp {
-
-struct GpError : std::runtime_error {
-  gp_status st;
-  GpError(gp_status s, const std::string& m) : std::runtime_error(m), st(s) {}
-};
-#define GP_CUDA(call)                                                                           \
-  do {                                                                                          \
-    cudaError_t e__ = (call);                                                                   \
-    if (e__ != cudaSuccess)                                                                     \
-      throw ::gp::GpError(GP_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e__));    \
-  } while (0)
-#define GP_REQUIRE(cond, msg)                                             \
-  do {                                                                    \
-    if (!(cond)) throw ::gp::GpError(GP_ERR_INVALID, std::string(msg));   \
-  } while (0)
 
 constexpr float kLatentScale = 0.18215f;   // genpercept_pipeline.py:96
 
@@ -317,13 +302,14 @@ void text_tower(Builder& b, WeightStore& ws, int n, const int32_t* ids, float* o
 // count the engines that share it (the last leave unmaps everything and frees the reservation); add maps enough for a
 // plan of `bytes` and returns the pool's fixed base, or null when the device cannot back it; remove gives a plan's share
 // back, synchronising the device before it unmaps.  wait / record order a call's stream after every earlier user of the
-// pool and every later user after the call.
+// pool and every later user after the call.  record runs as a call's use of the arena ends, on a throw too, so it never
+// throws: a failed record is left to the call's own CUDA error.
 void shared_arena_join(int device);
 void shared_arena_leave(int device);
 uint8_t* shared_arena_add(int device, size_t bytes);
 void shared_arena_remove(int device, size_t bytes);
 void shared_arena_wait(int device, cudaStream_t s);
-void shared_arena_record(int device, cudaStream_t s);
+void shared_arena_record(int device, cudaStream_t s) noexcept;
 
 // builder.cu: (BN, MT) of a stride-1 implicit-GEMM layer (default policy + the waves / L2-traffic model)
 // N tile width for a GEMM with `cout` output columns (`force` != 0: that width); one of 16, 32, 64, 128.

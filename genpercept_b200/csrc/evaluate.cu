@@ -13,6 +13,7 @@
 
 #include "launch.h"
 #include "prepost.h"
+#include "status.h"
 
 namespace gp {
 namespace {
@@ -240,7 +241,7 @@ __global__ void __launch_bounds__(kThreads) metrics_finish_kernel(const double* 
 // Blocks per image: about four pixels per thread, at most ~8 blocks per SM over the whole batch.
 int blocks_per_image(long long work, int B) {
   int dev = 0, sms = 132;
-  prepost_ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+  GP_CUDA(cudaGetDevice(&dev));
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long want = (work + kThreads * 4 - 1) / (kThreads * 4);
   const long long cap = ((long long)sms * 8 + B - 1) / B;
@@ -248,8 +249,7 @@ int blocks_per_image(long long work, int B) {
 }
 
 void check_shape(const char* fn, const void* pred, const void* gt, int B, int H, int W) {
-  if (!pred || !gt || B < 1 || B > 65535 || H < 1 || W < 1)
-    throw std::invalid_argument(std::string(fn) + ": bad arguments");
+  GP_REQUIRE(pred && gt && B >= 1 && B <= 65535 && H >= 1 && W >= 1, std::string(fn) + ": bad arguments");
 }
 
 }  // namespace
@@ -261,10 +261,9 @@ extern "C" {
 
 gp_status gp_depth_align(const float* pred, const float* gt, const uint8_t* valid, int B, int H, int W, int mode,
                          int max_res, float* scale_shift_out, float* aligned_out, void* stream) {
-  return prepost_guarded([&]() {
+  return guarded_call([&]() {
     check_shape("gp_depth_align", pred, gt, B, H, W);
-    if (!scale_shift_out || (mode != 0 && mode != 1) || max_res < 0)
-      throw std::invalid_argument("gp_depth_align: bad arguments");
+    GP_REQUIRE(scale_shift_out && (mode == 0 || mode == 1) && max_res >= 0, "gp_depth_align: bad arguments");
     // align_depth_least_square (alignment.py:43-53): s = min(max_res / (H, W)) in fp64; below 1 the fit grid is
     // H x floor(W * s) (the output size torch computes for a 1-D nearest upsample).
     int fit_w = W;
@@ -276,43 +275,40 @@ gp_status gp_depth_align(const float* pred, const float* gt, const uint8_t* vali
         inv_scale = (float)(1.0 / s);
       }
     }
-    if (fit_w < 1) throw std::invalid_argument("gp_depth_align: max_res leaves an empty fit grid");
+    GP_REQUIRE(fit_w >= 1, "gp_depth_align: max_res leaves an empty fit grid");
     std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
-    prepost_ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+    GP_CUDA(cudaGetDevice(&dev));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const int nblk = blocks_per_image((long long)H * fit_w, B);
     double* partials = static_cast<double*>(prepost_scratch(dev, (size_t)B * nblk * kAlignSlots * sizeof(double)));
-    prepost_ck(launch(align_stats_kernel, dim3(nblk, B), dim3(kThreads), 0, s, pred, gt, valid, H, W, mode, fit_w, inv_scale,
-                      partials), "align_stats_kernel");
-    prepost_ck(launch(align_solve_kernel, dim3(B), dim3(kThreads), 0, s, partials, nblk, scale_shift_out),
-               "align_solve_kernel");
+    GP_CUDA(launch(align_stats_kernel, dim3(nblk, B), dim3(kThreads), 0, s, pred, gt, valid, H, W, mode, fit_w, inv_scale,
+                   partials));
+    GP_CUDA(launch(align_solve_kernel, dim3(B), dim3(kThreads), 0, s, partials, nblk, scale_shift_out));
     if (aligned_out) {
       const long long npix = (long long)H * W, total = npix * B;
       const int g = blocks_per_image(total, 1);
-      prepost_ck(launch(apply_alignment_kernel, dim3(g), dim3(kThreads), 0, s, pred, scale_shift_out, npix, total,
-                        aligned_out), "apply_alignment_kernel");
+      GP_CUDA(launch(apply_alignment_kernel, dim3(g), dim3(kThreads), 0, s, pred, scale_shift_out, npix, total,
+                     aligned_out));
     }
   });
 }
 
 gp_status gp_depth_metrics(const float* pred, const float* gt, const uint8_t* valid, int B, int H, int W, int mode,
                            const float* scale_shift, float min_depth, float max_depth, double* metrics_out, void* stream) {
-  return prepost_guarded([&]() {
+  return guarded_call([&]() {
     check_shape("gp_depth_metrics", pred, gt, B, H, W);
-    if (!metrics_out || mode < 0 || mode > 2 || (mode != 0 && !scale_shift))
-      throw std::invalid_argument("gp_depth_metrics: bad arguments");
+    GP_REQUIRE(metrics_out && mode >= 0 && mode <= 2 && (mode == 0 || scale_shift), "gp_depth_metrics: bad arguments");
     std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
-    prepost_ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+    GP_CUDA(cudaGetDevice(&dev));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const long long npix = (long long)H * W;
     const int nblk = blocks_per_image(npix, B);
     double* partials = static_cast<double*>(prepost_scratch(dev, (size_t)B * nblk * kMetricSlots * sizeof(double)));
-    prepost_ck(launch(metrics_kernel, dim3(nblk, B), dim3(kThreads), 0, s, pred, gt, valid, npix, mode, scale_shift,
-                      min_depth, max_depth, partials), "metrics_kernel");
-    prepost_ck(launch(metrics_finish_kernel, dim3(B), dim3(kThreads), 0, s, partials, nblk, metrics_out),
-               "metrics_finish_kernel");
+    GP_CUDA(launch(metrics_kernel, dim3(nblk, B), dim3(kThreads), 0, s, pred, gt, valid, npix, mode, scale_shift,
+                   min_depth, max_depth, partials));
+    GP_CUDA(launch(metrics_finish_kernel, dim3(B), dim3(kThreads), 0, s, partials, nblk, metrics_out));
   });
 }
 

@@ -17,12 +17,12 @@
 
 #include <map>
 #include <mutex>
-#include <stdexcept>
 #include <string>
 #include <tuple>
 #include <vector>
 
 #include "prepost.h"
+#include "status.h"
 
 namespace gp {
 namespace {
@@ -131,14 +131,12 @@ std::map<std::tuple<int, int, int, int>, AxisTable> g_tables;     // (device, in
 struct Scratch { void* p = nullptr; size_t bytes = 0; };
 std::map<int, Scratch> g_scratch;                                   // per device, grows
 
-void ck(cudaError_t e, const char* what) { prepost_ck(e, what); }
-
 const AxisTable& axis_table(int dev, int in_size, int out_size, int mode) {
   auto key = std::make_tuple(dev, in_size, out_size, mode);
   auto it = g_tables.find(key);
   if (it != g_tables.end()) return it->second;
   if (g_tables.size() >= 64) {   // every distinct (in, out) extent is a table: bound the cache (a folder of in-the-wild images)
-    ck(cudaDeviceSynchronize(), "cudaDeviceSynchronize");
+    GP_CUDA(cudaDeviceSynchronize());
     for (auto& kv : g_tables) {
       cudaFree(kv.second.xmin);
       cudaFree(kv.second.xsize);
@@ -160,16 +158,16 @@ const AxisTable& axis_table(int dev, int in_size, int out_size, int mode) {
   } else {
     build_axis(in_size, out_size, mode, xmin, xsize, w, &t.kmax);
   }
-  ck(cudaMalloc(reinterpret_cast<void**>(&t.xmin), xmin.size() * 4), "cudaMalloc");
-  ck(cudaMalloc(reinterpret_cast<void**>(&t.xsize), xsize.size() * 4), "cudaMalloc");
-  ck(cudaMemcpy(t.xmin, xmin.data(), xmin.size() * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
-  ck(cudaMemcpy(t.xsize, xsize.data(), xsize.size() * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
+  GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&t.xmin), xmin.size() * 4));
+  GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&t.xsize), xsize.size() * 4));
+  GP_CUDA(cudaMemcpy(t.xmin, xmin.data(), xmin.size() * 4, cudaMemcpyHostToDevice));
+  GP_CUDA(cudaMemcpy(t.xsize, xsize.data(), xsize.size() * 4, cudaMemcpyHostToDevice));
   if (mode == 2) {
-    ck(cudaMalloc(reinterpret_cast<void**>(&t.wq), wq.size() * 4), "cudaMalloc");
-    ck(cudaMemcpy(t.wq, wq.data(), wq.size() * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
+    GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&t.wq), wq.size() * 4));
+    GP_CUDA(cudaMemcpy(t.wq, wq.data(), wq.size() * 4, cudaMemcpyHostToDevice));
   } else {
-    ck(cudaMalloc(reinterpret_cast<void**>(&t.w), w.size() * 4), "cudaMalloc");
-    ck(cudaMemcpy(t.w, w.data(), w.size() * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
+    GP_CUDA(cudaMalloc(reinterpret_cast<void**>(&t.w), w.size() * 4));
+    GP_CUDA(cudaMemcpy(t.w, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
   }
   return g_tables.emplace(key, t).first->second;
 }
@@ -450,10 +448,10 @@ std::mutex& prepost_mutex() {
 void* prepost_scratch(int dev, size_t bytes) {
   Scratch& s = g_scratch[dev];
   if (s.bytes < bytes) {
-    if (s.p) ck(cudaFree(s.p), "cudaFree");
+    if (s.p) GP_CUDA(cudaFree(s.p));
     s.p = nullptr;
     s.bytes = 0;
-    ck(cudaMalloc(&s.p, bytes), "cudaMalloc");
+    GP_CUDA(cudaMalloc(&s.p, bytes));
     s.bytes = bytes;
   }
   return s.p;
@@ -467,13 +465,13 @@ extern "C" {
 
 gp_status gp_resize_aa(const void* src, int src_dtype, int src_on_host, int N, int H, int W, void* dst, int dst_dtype,
                        int dst_on_host, int OH, int OW, int mode, void* stream) {
-  return prepost_guarded([&]() {
-    if (!src || !dst || N < 1 || H < 1 || W < 1 || OH < 1 || OW < 1 || (mode != 0 && mode != 1) ||
-        (src_dtype != GP_U8 && src_dtype != GP_F32) || (dst_dtype != GP_U8 && dst_dtype != GP_F32))
-      throw std::invalid_argument("gp_resize_aa: bad arguments");
+  return guarded_call([&]() {
+    GP_REQUIRE(src && dst && N >= 1 && H >= 1 && W >= 1 && OH >= 1 && OW >= 1 && (mode == 0 || mode == 1) &&
+                   (src_dtype == GP_U8 || src_dtype == GP_F32) && (dst_dtype == GP_U8 || dst_dtype == GP_F32),
+               "gp_resize_aa: bad arguments");
     std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
-    ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+    GP_CUDA(cudaGetDevice(&dev));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const size_t n_in = (size_t)N * H * W, n_mid = (size_t)N * H * OW, n_out = (size_t)N * OH * OW;
     // scratch layout: [staged input][width-pass result f32][staged output]
@@ -483,7 +481,7 @@ gp_status gp_resize_aa(const void* src, int src_dtype, int src_on_host, int N, i
     uint8_t* sc = static_cast<uint8_t*>(prepost_scratch(dev, in_b + mid_b + out_b));
     const void* d_src = src;
     if (src_on_host) {
-      ck(cudaMemcpyAsync(sc, src, n_in * esize(src_dtype), cudaMemcpyHostToDevice, s), "H2D");
+      GP_CUDA(cudaMemcpyAsync(sc, src, n_in * esize(src_dtype), cudaMemcpyHostToDevice, s));
       d_src = sc;
     }
     float* mid = reinterpret_cast<float*>(sc + in_b);
@@ -501,7 +499,7 @@ gp_status gp_resize_aa(const void* src, int src_dtype, int src_on_host, int N, i
       if (src_dtype == GP_U8) cast_copy<uint8_t><<<g, 256, 0, s>>>(static_cast<const uint8_t*>(d_src), mid, (long long)n_mid);
       else cast_copy<float><<<g, 256, 0, s>>>(static_cast<const float*>(d_src), mid, (long long)n_mid);
     }
-    ck(cudaGetLastError(), "aa width pass");
+    GP_CUDA(cudaGetLastError());
     // height pass (identity table when the height is unchanged: window of one tap, weight 1)
     const AxisTable& th = axis_table(dev, H, OH, H == OH ? 0 : mode);
     const int g = grid_for((long long)n_out, dev);
@@ -510,45 +508,44 @@ gp_status gp_resize_aa(const void* src, int src_dtype, int src_on_host, int N, i
       aa_pass_h<uint8_t><<<g, 256, 0, s>>>(mid, static_cast<uint8_t*>(d_dst), N, H, OH, OW, th.xmin, th.xsize, th.w, th.kmax, clamp);
     else
       aa_pass_h<float><<<g, 256, 0, s>>>(mid, static_cast<float*>(d_dst), N, H, OH, OW, th.xmin, th.xsize, th.w, th.kmax, 0);
-    ck(cudaGetLastError(), "aa height pass");
-    if (dst_on_host) ck(cudaMemcpyAsync(dst, d_dst, n_out * esize(dst_dtype), cudaMemcpyDeviceToHost, s), "D2H");
-    if (src_on_host || dst_on_host) ck(cudaStreamSynchronize(s), "sync");
+    GP_CUDA(cudaGetLastError());
+    if (dst_on_host) GP_CUDA(cudaMemcpyAsync(dst, d_dst, n_out * esize(dst_dtype), cudaMemcpyDeviceToHost, s));
+    if (src_on_host || dst_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }
 
 gp_status gp_colorize(const float* pred, int pred_on_host, int B, int H, int W, float vmin, float vmax,
                       const uint8_t* lut768_host, uint8_t* out_hwc, int out_on_host, void* stream) {
-  return prepost_guarded([&]() {
-    if (!pred || !lut768_host || !out_hwc || B < 1 || H < 1 || W < 1 || !(vmax > vmin))
-      throw std::invalid_argument("gp_colorize: bad arguments");
+  return guarded_call([&]() {
+    GP_REQUIRE(pred && lut768_host && out_hwc && B >= 1 && H >= 1 && W >= 1 && vmax > vmin, "gp_colorize: bad arguments");
     std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
-    ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+    GP_CUDA(cudaGetDevice(&dev));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const size_t n = (size_t)B * H * W;
     const size_t in_b = pred_on_host ? (n * 4 + 255) / 256 * 256 : 0;
     const size_t out_b = out_on_host ? (n * 3 + 255) / 256 * 256 : 0;
     uint8_t* sc = static_cast<uint8_t*>(prepost_scratch(dev, 1024 + in_b + out_b));
-    ck(cudaMemcpyAsync(sc, lut768_host, 768, cudaMemcpyHostToDevice, s), "lut H2D");
+    GP_CUDA(cudaMemcpyAsync(sc, lut768_host, 768, cudaMemcpyHostToDevice, s));
     const float* d_pred = pred;
     if (pred_on_host) {
-      ck(cudaMemcpyAsync(sc + 1024, pred, n * 4, cudaMemcpyHostToDevice, s), "H2D");
+      GP_CUDA(cudaMemcpyAsync(sc + 1024, pred, n * 4, cudaMemcpyHostToDevice, s));
       d_pred = reinterpret_cast<const float*>(sc + 1024);
     }
     uint8_t* d_out = out_on_host ? sc + 1024 + in_b : out_hwc;
     colorize_kernel<<<grid_for((long long)n, dev), 256, 0, s>>>(d_pred, d_out, (long long)n, vmin, vmax - vmin, sc);
-    ck(cudaGetLastError(), "colorize");
-    if (out_on_host) ck(cudaMemcpyAsync(out_hwc, d_out, n * 3, cudaMemcpyDeviceToHost, s), "D2H");
-    ck(cudaStreamSynchronize(s), "sync");                  // the host LUT buffer may be released by the caller
+    GP_CUDA(cudaGetLastError());
+    if (out_on_host) GP_CUDA(cudaMemcpyAsync(out_hwc, d_out, n * 3, cudaMemcpyDeviceToHost, s));
+    GP_CUDA(cudaStreamSynchronize(s));                  // the host LUT buffer may be released by the caller
   });
 }
 
 gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, void* out, int out_on_host, void* stream) {
-  return prepost_guarded([&]() {
-    if (!pred || !out || n < 1 || (bits != 8 && bits != 16)) throw std::invalid_argument("gp_quantize: bad arguments");
+  return guarded_call([&]() {
+    GP_REQUIRE(pred && out && n >= 1 && (bits == 8 || bits == 16), "gp_quantize: bad arguments");
     std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
-    ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+    GP_CUDA(cudaGetDevice(&dev));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const size_t ob = bits / 8;
     const size_t in_b = pred_on_host ? (n * 4 + 255) / 256 * 256 : 0;
@@ -556,24 +553,24 @@ gp_status gp_quantize(const float* pred, int pred_on_host, size_t n, int bits, v
     uint8_t* sc = (in_b + out_b) ? static_cast<uint8_t*>(prepost_scratch(dev, in_b + out_b)) : nullptr;
     const float* d_pred = pred;
     if (pred_on_host) {
-      ck(cudaMemcpyAsync(sc, pred, n * 4, cudaMemcpyHostToDevice, s), "H2D");
+      GP_CUDA(cudaMemcpyAsync(sc, pred, n * 4, cudaMemcpyHostToDevice, s));
       d_pred = reinterpret_cast<const float*>(sc);
     }
     void* d_out = out_on_host ? static_cast<void*>(sc + in_b) : out;
     quantize_kernel<<<grid_for((long long)n, dev), 256, 0, s>>>(d_pred, d_out, (long long)n, bits);
-    ck(cudaGetLastError(), "quantize");
-    if (out_on_host) ck(cudaMemcpyAsync(out, d_out, n * ob, cudaMemcpyDeviceToHost, s), "D2H");
-    if (pred_on_host || out_on_host) ck(cudaStreamSynchronize(s), "sync");
+    GP_CUDA(cudaGetLastError());
+    if (out_on_host) GP_CUDA(cudaMemcpyAsync(out, d_out, n * ob, cudaMemcpyDeviceToHost, s));
+    if (pred_on_host || out_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }
 
 gp_status gp_resize_pil(const uint8_t* src_hwc, int src_on_host, int H, int W, uint8_t* dst_chw, int dst_on_host, int OH,
                         int OW, void* stream) {
-  return prepost_guarded([&]() {
-    if (!src_hwc || !dst_chw || H < 1 || W < 1 || OH < 1 || OW < 1) throw std::invalid_argument("gp_resize_pil: bad arguments");
+  return guarded_call([&]() {
+    GP_REQUIRE(src_hwc && dst_chw && H >= 1 && W >= 1 && OH >= 1 && OW >= 1, "gp_resize_pil: bad arguments");
     std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
-    ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+    GP_CUDA(cudaGetDevice(&dev));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     // the rows the vertical pass reads (Pillow: ybox_first .. ybox_last); all of them when the height is kept
     int row0 = 0, rows = H;
@@ -590,7 +587,7 @@ gp_status gp_resize_pil(const uint8_t* src_hwc, int src_on_host, int H, int W, u
     uint8_t* sc = (in_b + mid_b + out_b) ? static_cast<uint8_t*>(prepost_scratch(dev, in_b + mid_b + out_b)) : nullptr;
     const uint8_t* d_src = src_hwc;
     if (src_on_host) {
-      ck(cudaMemcpyAsync(sc, src_hwc, n_in, cudaMemcpyHostToDevice, s), "H2D");
+      GP_CUDA(cudaMemcpyAsync(sc, src_hwc, n_in, cudaMemcpyHostToDevice, s));
       d_src = sc;
     }
     uint8_t* d_dst = dst_on_host ? sc + in_b + mid_b : dst_chw;
@@ -599,32 +596,32 @@ gp_status gp_resize_pil(const uint8_t* src_hwc, int src_on_host, int H, int W, u
       const AxisTable& th = axis_table(dev, W, OW, 2);
       uint8_t* mid = sc + in_b;
       pil_pass_h<<<grid_for((long long)rows * OW, dev), 256, 0, s>>>(cur, mid, rows, W, OW, th.xmin, th.xsize, th.wq, th.kmax);
-      ck(cudaGetLastError(), "pil horizontal pass");
+      GP_CUDA(cudaGetLastError());
       cur = mid;
     }
     if (H != OH) {   // looked up again: the width table's insertion may have evicted it (the cache is bounded)
       const AxisTable& tv = axis_table(dev, H, OH, 2);
       pil_pass_v<<<grid_for((long long)OH * OW, dev), 256, 0, s>>>(cur, d_dst, OH, OW, row0, tv.xmin, tv.xsize, tv.wq, tv.kmax);
-      ck(cudaGetLastError(), "pil vertical pass");
+      GP_CUDA(cudaGetLastError());
     } else {
       hwc_to_chw<<<grid_for((long long)OH * OW, dev), 256, 0, s>>>(cur, d_dst, (long long)OH * OW);
-      ck(cudaGetLastError(), "hwc_to_chw");
+      GP_CUDA(cudaGetLastError());
     }
-    if (dst_on_host) ck(cudaMemcpyAsync(dst_chw, d_dst, n_out, cudaMemcpyDeviceToHost, s), "D2H");
-    if (src_on_host || dst_on_host) ck(cudaStreamSynchronize(s), "sync");
+    if (dst_on_host) GP_CUDA(cudaMemcpyAsync(dst_chw, d_dst, n_out, cudaMemcpyDeviceToHost, s));
+    if (src_on_host || dst_on_host) GP_CUDA(cudaStreamSynchronize(s));
   });
 }
 
 gp_status gp_v1_postprocess(const float* pred, int B, int C, int h, int w, int task, int H, int W, float* out_f32,
                             uint8_t* out_u8, void* stream) {
-  return prepost_guarded([&]() {
+  return guarded_call([&]() {
     const bool ok = pred && B >= 1 && h >= 1 && w >= 1 && H >= 1 && W >= 1 &&
                     ((task == 0 && C == 1 && out_f32) || (task == 1 && C == 3 && out_f32 && out_u8) ||
                      (task == 2 && C == 3 && out_u8));
-    if (!ok) throw std::invalid_argument("gp_v1_postprocess: bad arguments");
+    GP_REQUIRE(ok, "gp_v1_postprocess: bad arguments");
     std::lock_guard<std::mutex> lock(prepost_mutex());
     int dev = 0;
-    ck(cudaGetDevice(&dev), "cudaGetDevice (no CUDA device: this library has no CPU path)");
+    GP_CUDA(cudaGetDevice(&dev));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     V1Interp g;
     g.h = h; g.w = w; g.H = H; g.W = W;
@@ -635,19 +632,19 @@ gp_status gp_v1_postprocess(const float* pred, int B, int C, int h, int w, int t
     if (task == 0) {
       long long parts = (n + 2047) / 2048;
       const int nparts = (int)(parts < 1 ? 1 : (parts > 256 ? 256 : parts));
-      if (B > 65535) throw std::invalid_argument("gp_v1_postprocess: batch above 65535");
+      GP_REQUIRE(B <= 65535, "gp_v1_postprocess: batch above 65535");
       float2* partial = static_cast<float2*>(prepost_scratch(dev, (size_t)B * nparts * sizeof(float2)));
       const dim3 grid(nparts, B);
       v1_depth_interp<<<grid, kV1Threads, 0, s>>>(pred, out_f32, g, partial);
-      ck(cudaGetLastError(), "v1 depth interpolation");
+      GP_CUDA(cudaGetLastError());
       v1_depth_normalise<<<grid, kV1Threads, 0, s>>>(out_f32, n, partial, nparts);
-      ck(cudaGetLastError(), "v1 depth normalisation");
+      GP_CUDA(cudaGetLastError());
     } else if (task == 1) {
       v1_normal<<<grid_for((long long)B * n, dev), 256, 0, s>>>(pred, out_f32, out_u8, g, B);
-      ck(cudaGetLastError(), "v1 normal");
+      GP_CUDA(cudaGetLastError());
     } else {
       v1_seg<<<grid_for((long long)B * 3 * n, dev), 256, 0, s>>>(pred, out_u8, g, B);
-      ck(cudaGetLastError(), "v1 seg");
+      GP_CUDA(cudaGetLastError());
     }
   });
 }

@@ -14,10 +14,9 @@
 #include <stdint.h>
 #include <string.h>
 
-#include <stdexcept>
 #include <string>
 
-#include "../../include/genpercept_b200.h"
+#include "status.h"
 
 namespace {
 
@@ -82,7 +81,7 @@ struct State {                      // device-side status block
 };
 
 // ------------------------------------------------------------------------------------------------ host parser
-[[noreturn]] void reject(const char* why) { throw std::invalid_argument(why); }
+[[noreturn]] void reject(const char* why) { throw gp::GpError(GP_ERR_INVALID, why); }
 
 void build_huff(const uint8_t* counts, const uint8_t* vals, int n, bool dc, HuffDev& t) {
   memset(&t, 0, sizeof t);
@@ -836,37 +835,14 @@ __global__ void __launch_bounds__(256) ycc_to_rgb(Geo g, const uint8_t* pix, uin
   }
 }
 
-thread_local std::string g_jpeg_error;
-
-template <typename F>
-gp_status jpeg_guarded(F f) {
-  try {
-    g_jpeg_error.clear();
-    f();
-    return GP_OK;
-  } catch (const std::invalid_argument& ex) {
-    g_jpeg_error = ex.what();
-    return GP_ERR_INVALID;
-  } catch (const std::exception& ex) {
-    g_jpeg_error = ex.what();
-    return GP_ERR_CUDA;
-  }
-}
-
-void ck(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
-}
-
 unsigned grid(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
 }  // namespace
 
 extern "C" {
 
-const char* gp_jpeg_last_error(void) { return g_jpeg_error.c_str(); }
-
 gp_status gp_jpeg_probe(const uint8_t* data, size_t nbytes, int* H, int* W, int64_t* workspace_bytes) {
-  return jpeg_guarded([&]() {
+  return gp::guarded_call([&]() {
     const Header hd = parse(data, nbytes);
     const Layout y = plan(hd, nbytes);
     if (H) *H = hd.H;
@@ -878,11 +854,11 @@ gp_status gp_jpeg_probe(const uint8_t* data, size_t nbytes, int* H, int* W, int6
 gp_status gp_jpeg_decode(const uint8_t* data_host, size_t nbytes, void* workspace_dev, int64_t workspace_bytes,
                          uint8_t* dst_dev, int64_t row_stride, int64_t pixel_stride, int64_t channel_stride,
                          void* stream) {
-  return jpeg_guarded([&]() {
+  return gp::guarded_call([&]() {
     const Header hd = parse(data_host, nbytes);
     const Layout y = plan(hd, nbytes);
-    if (!workspace_dev || workspace_bytes < (int64_t)y.total) throw std::invalid_argument("workspace too small");
-    if (!dst_dev) throw std::invalid_argument("no output buffer");
+    GP_REQUIRE(workspace_dev && workspace_bytes >= (int64_t)y.total, "workspace too small");
+    GP_REQUIRE(dst_dev, "no output buffer");
     const Geo& g = y.g;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     uint8_t* ws = static_cast<uint8_t*>(workspace_dev);
@@ -905,12 +881,12 @@ gp_status gp_jpeg_decode(const uint8_t* data_host, size_t nbytes, void* workspac
     State init;
     memset(&init, 0, sizeof init);
     init.end = (int)y.L;
-    ck(cudaMemcpyAsync(at(y.o_file), data_host, nbytes, cudaMemcpyHostToDevice, s), "upload");
-    ck(cudaMemcpyAsync(at(y.o_tab), &hd.t, sizeof(Tables), cudaMemcpyHostToDevice, s), "upload tables");
-    ck(cudaMemcpyAsync(st, &init, sizeof init, cudaMemcpyHostToDevice, s), "upload state");
-    ck(cudaMemsetAsync(U, 0, y.o_rst - y.o_u, s), "memset");
-    ck(cudaMemsetAsync(rst, 0, (size_t)g.n_int * 4, s), "memset");
-    ck(cudaMemsetAsync(coef, 0, (size_t)y.coef_elems * 2, s), "memset");
+    GP_CUDA(cudaMemcpyAsync(at(y.o_file), data_host, nbytes, cudaMemcpyHostToDevice, s));
+    GP_CUDA(cudaMemcpyAsync(at(y.o_tab), &hd.t, sizeof(Tables), cudaMemcpyHostToDevice, s));
+    GP_CUDA(cudaMemcpyAsync(st, &init, sizeof init, cudaMemcpyHostToDevice, s));
+    GP_CUDA(cudaMemsetAsync(U, 0, y.o_rst - y.o_u, s));
+    GP_CUDA(cudaMemsetAsync(rst, 0, (size_t)g.n_int * 4, s));
+    GP_CUDA(cudaMemsetAsync(coef, 0, (size_t)y.coef_elems * 2, s));
 
     find_end<<<grid(y.L, 256 * 16), 256, 0, s>>>(E, y.L, st);
     unstuff_count<<<(unsigned)y.n_chunks, 256, 0, s>>>(E, y.L, st, chunks, at(y.o_chunk_f));
@@ -930,8 +906,8 @@ gp_status gp_jpeg_decode(const uint8_t* data_host, size_t nbytes, void* workspac
                                                          exits, agg);
       last = pass + kPassBatch - 1;
       int changed = 1;
-      ck(cudaMemcpyAsync(&changed, &st->changed[last], sizeof changed, cudaMemcpyDeviceToHost, s), "flag");
-      ck(cudaStreamSynchronize(s), "sync");
+      GP_CUDA(cudaMemcpyAsync(&changed, &st->changed[last], sizeof changed, cudaMemcpyDeviceToHost, s));
+      GP_CUDA(cudaStreamSynchronize(s));
       if (!changed) break;
     }
     scan(agg, at(y.o_agg_f), y.n_sub_max, reinterpret_cast<S4*>(at(y.o_agg_b)), at(y.o_agg_bf), s);
@@ -939,10 +915,10 @@ gp_status gp_jpeg_decode(const uint8_t* data_host, size_t nbytes, void* workspac
     idct_islow<<<grid(y.n_blocks, kIdctBlocks), 256, 0, s>>>(tab, g, coef, pix, y.n_blocks, st);
     ycc_to_rgb<<<grid((long long)g.W * g.H, 256), 256, 0, s>>>(g, pix, dst_dev, row_stride, pixel_stride,
                                                               channel_stride, st);
-    ck(cudaGetLastError(), "jpeg kernels");
+    GP_CUDA(cudaGetLastError());
     State out;
-    ck(cudaMemcpyAsync(&out, st, sizeof out, cudaMemcpyDeviceToHost, s), "status");
-    ck(cudaStreamSynchronize(s), "sync");
+    GP_CUDA(cudaMemcpyAsync(&out, st, sizeof out, cudaMemcpyDeviceToHost, s));
+    GP_CUDA(cudaStreamSynchronize(s));
     if (out.status == 0 && out.blocks_done != (unsigned long long)y.n_blocks) out.status = ST_COUNT;
     if (out.status) {
       static const char* why[] = {"unexpected marker or no EOI in the scan", "restart markers out of sequence",
@@ -952,7 +928,7 @@ gp_status gp_jpeg_decode(const uint8_t* data_host, size_t nbytes, void* workspac
                                   "IDCT value outside the range libjpeg-turbo's C and SIMD IDCTs agree on"};
       int bit = 0;
       while (!(out.status >> bit & 1)) ++bit;
-      throw std::invalid_argument(std::string("corrupt or undecodable JPEG stream: ") + why[bit]);
+      throw gp::GpError(GP_ERR_INVALID, std::string("corrupt or undecodable JPEG stream: ") + why[bit]);
     }
   });
 }

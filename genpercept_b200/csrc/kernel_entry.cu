@@ -1,7 +1,6 @@
 // Per-kernel entry points of the C-ABI: one layer at a time on caller buffers, for the parity tests and the
 // micro-benchmarks.  Weights go through a throwaway WeightStore and the ops through the Builder, so these run the
 // engine's own packing and launch paths.
-#include <cstdio>
 #include <cstring>
 
 #include "engine.h"
@@ -9,20 +8,6 @@
 using namespace gp;
 
 namespace {
-
-template <class F>
-gp_status guarded_free(F f) {
-  try {
-    f();
-    return GP_OK;
-  } catch (const GpError& ex) {
-    fprintf(stderr, "[genpercept_b200] %s\n", ex.what());
-    return ex.st;
-  } catch (const std::exception& ex) {
-    fprintf(stderr, "[genpercept_b200] %s\n", ex.what());
-    return GP_ERR_INVALID;
-  }
-}
 
 void run_all(Builder& b, cudaStream_t s) {
   for (auto& op : b.ops) GP_CUDA(op.run(s));
@@ -90,7 +75,7 @@ extern "C" {
 
 gp_status gp_conv2d(int dtype, const void* x, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
                     int Cout, int ks, int mode, const void* residual, int relu, void* y, int use_direct, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && w_host && y && (ks == 1 || ks == 3) && mode >= 0 && mode <= 3, "gp_conv2d: bad arguments");
     const bool pair = storage_layout(dtype, true, "gp_conv2d");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -139,7 +124,7 @@ gp_status gp_conv2d(int dtype, const void* x, int N, int H, int W, int Cin, cons
 
 gp_status gp_groupnorm(int dtype, const void* x, int N, int H, int W, int C, int groups, const float* gamma_host,
                        const float* beta_host, float eps, int silu, void* y, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && y && gamma_host && beta_host && groups >= 1 && C % groups == 0 && C % 8 == 0, "gp_groupnorm: bad arguments");
     const bool pair = storage_layout(dtype, true, "gp_groupnorm");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -159,7 +144,7 @@ gp_status gp_gn_conv3x3(int dtype, const void* x, int N, int H, int W, int Cin, 
                         const float* beta_host, float eps, int silu, const float* w_host, const float* bias_host, int Cout,
                         const void* sc_x, int Csc, const float* sc_w_host, const float* sc_b_host, const void* residual,
                         void* y, int out_f32, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && w_host && y && gamma_host && beta_host, "gp_gn_conv3x3: bad arguments");
     const bool pair = storage_layout(dtype, true, "gp_gn_conv3x3");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -196,7 +181,7 @@ gp_status gp_gn_conv3x3(int dtype, const void* x, int N, int H, int W, int Cin, 
 gp_status gp_conv_groupnorm(int dtype, const void* x, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
                             int Cout, const void* skip, int Cskip, int groups, const float* gamma_host, const float* beta_host,
                             float eps, int silu, void* y_conv, void* y, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && w_host && y_conv && y && gamma_host && beta_host && groups >= 1 && Cout % 8 == 0 && Cskip % 8 == 0 &&
                    (skip ? Cskip > 0 : Cskip == 0) && (Cout + Cskip) % groups == 0,
                "gp_conv_groupnorm: bad arguments");
@@ -229,7 +214,7 @@ gp_status gp_conv_groupnorm(int dtype, const void* x, int N, int H, int W, int C
 
 gp_status gp_layernorm(int dtype, const void* x, int64_t tokens, int C, const float* gamma_host, const float* beta_host,
                        float eps, void* y, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && y && gamma_host && beta_host && tokens >= 0 && C >= 8, "gp_layernorm: bad arguments");
     const bool pair = storage_layout(dtype, true, "gp_layernorm");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -243,7 +228,7 @@ gp_status gp_layernorm(int dtype, const void* x, int64_t tokens, int C, const fl
 
 gp_status gp_attention(int dtype, const void* q, const void* k, const void* v, int B, int T, int heads, int d, float scale,
                        void* o, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     // q is pre-scaled by the caller-visible `scale` through an identity-weight GEMM, and V^T is the engine's own
     // swapped-operand GEMM with identity weights, so that the same igemm paths the engine uses (QK^T, softmax, V^T, PV)
     // are exercised.
@@ -267,7 +252,7 @@ gp_status gp_attention(int dtype, const void* q, const void* k, const void* v, i
 }
 
 gp_status gp_attention_high(const void* qk, const void* v, int B, int T, int heads, int d, int fused, void* o, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(qk && v && o && B >= 1 && T >= 1 && (d == 64 || (d == 512 && heads == 1)),
                "gp_attention_high: bad arguments (d = 64, or d = 512 with one head)");
     // V^T is the engine's swapped-operand GEMM with identity weights (hi 1, lo 0), which reproduces v's (hi, lo) pairs
@@ -290,7 +275,7 @@ gp_status gp_attention_high(const void* qk, const void* v, int B, int T, int hea
 
 gp_status gp_ensemble_reduce(const float* pred_dev, int B, int H, int W, const float* scale_host, const float* shift_host,
                              int median, int normalise, float* out_dev, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(pred_dev && out_dev && scale_host && shift_host && B >= 1 && B <= 32, "gp_ensemble_reduce: bad arguments (B <= 32)");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     float* ss = nullptr;
@@ -310,7 +295,7 @@ gp_status gp_ensemble_reduce(const float* pred_dev, int B, int H, int W, const f
 }
 
 gp_status gp_bilinear_up2x(int dtype, const void* x, int N, int H, int W, int C, void* y, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && y && N >= 1 && H >= 1 && W >= 1 && C >= 1, "gp_bilinear_up2x: bad arguments");
     const bool pair = storage_layout(dtype, true, "gp_bilinear_up2x");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -321,7 +306,7 @@ gp_status gp_bilinear_up2x(int dtype, const void* x, int N, int H, int W, int C,
 
 gp_status gp_geglu(int dtype, const void* x, int64_t tokens, int C, const float* w_host, const float* b_host, void* y,
                    void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && y && w_host && b_host && tokens >= 1 && tokens < (1LL << 31) && C >= 8 && C % 8 == 0,
                "gp_geglu: bad arguments (C % 8 == 0)");
     const bool pair = storage_layout(dtype, true, "gp_geglu");
@@ -339,7 +324,7 @@ gp_status gp_cross_attention(int dtype, const void* x, int64_t tokens, int C, in
                              const float* to_q, const float* to_k, const float* to_v, const float* to_out_w,
                              const float* to_out_b, const float* norm_g, const float* norm_b, float eps, void* y,
                              void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && y && ctx_host && to_q && to_k && to_v && to_out_w && to_out_b && norm_g && norm_b && tokens >= 1 &&
                    tokens < (1LL << 31) && heads >= 1 && C % heads == 0 && C % 8 == 0 && n >= 1 && E >= 1,
                "gp_cross_attention: bad arguments (C % 8 == 0, C % heads == 0)");
@@ -366,7 +351,7 @@ gp_status gp_resnet(int dtype, const void* x, int Cx, const void* skip, int Cski
                     const float* norm1_g, const float* norm1_b, const float* conv1_w, const float* conv1_b,
                     const float* norm2_g, const float* norm2_b, const float* conv2_w, const float* conv2_b,
                     const float* shortcut_w, const float* shortcut_b, void* y, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     const int Cin = Cx + Cskip;
     GP_REQUIRE(x && y && norm1_g && norm1_b && conv1_w && conv1_b && norm2_g && norm2_b && conv2_w && conv2_b && N >= 1 &&
                    H >= 1 && W >= 1 && Cx >= 8 && Cx % 8 == 0 && Cskip % 8 == 0 && (skip ? Cskip > 0 : Cskip == 0) &&
@@ -408,7 +393,7 @@ gp_status gp_resnet(int dtype, const void* x, int Cx, const void* skip, int Cski
 }
 
 gp_status gp_resize(int dtype, const void* x, int N, int H, int W, int C, int OH, int OW, int mode, void* y, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && y && N >= 1 && H >= 1 && W >= 1 && OH >= 1 && OW >= 1 && C >= 8 && C % 8 == 0 && (mode == 0 || mode == 1),
                "gp_resize: bad arguments (C % 8 == 0, mode 0 nearest or 1 bilinear)");
     const bool pair = storage_layout(dtype, true, "gp_resize");
@@ -421,7 +406,7 @@ gp_status gp_resize(int dtype, const void* x, int N, int H, int W, int C, int OH
 }
 
 gp_status gp_causal_attention(int dtype, const void* qkv, int n, int heads, int d, void* out, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(qkv && out && n >= 1 && n <= kTextMaxTokens && heads >= 1 && d >= 1 && d <= kCausalMaxD,
                "gp_causal_attention: bad arguments (1 <= n <= 77, 1 <= d <= 64)");
     const bool pair = storage_layout(dtype, true, "gp_causal_attention");
@@ -432,7 +417,7 @@ gp_status gp_causal_attention(int dtype, const void* qkv, int n, int heads, int 
 }
 
 gp_status gp_gelu(int dtype, const void* x, int64_t n_elems, void* y, void* stream) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(x && y && n_elems >= 8 && n_elems % 8 == 0 && n_elems < (1LL << 30), "gp_gelu: bad arguments (n_elems % 8 == 0)");
     const bool pair = storage_layout(dtype, true, "gp_gelu");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -443,7 +428,7 @@ gp_status gp_gelu(int dtype, const void* x, int64_t n_elems, void* y, void* stre
 
 gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int ks, int mode, int iters, double* usec,
                         double* flops) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     storage_layout(dtype, false, "gp_bench_conv");
     WeightStore ws(dtype == GP_BF16);
     const std::vector<float> wt((size_t)Cout * Cin * ks * ks, 0.01f), bz(Cout, 0.f);
@@ -468,7 +453,7 @@ gp_status gp_bench_conv(int dtype, int N, int H, int W, int Cin, int Cout, int k
 }
 
 gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, double* usec, double* flops) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     storage_layout(dtype, false, "gp_bench_attention");
     GP_REQUIRE(B >= 1 && T >= 1 && iters >= 1, "gp_bench_attention: bad arguments");
     WeightStore ws(dtype == GP_BF16);
@@ -493,7 +478,7 @@ gp_status gp_bench_attention(int dtype, int B, int T, int fused, int iters, doub
 }
 
 gp_status gp_bench_attention_high(int B, int T, int heads, int d, int fused, int iters, double* usec, double* flops) {
-  return guarded_free([&]() {
+  return guarded_call([&]() {
     GP_REQUIRE(B >= 1 && T >= 1 && iters >= 1 && (d == 64 || (d == 512 && heads == 1)),
                "gp_bench_attention_high: bad arguments (d = 64, or d = 512 with one head)");
     WeightStore ws(false, true);

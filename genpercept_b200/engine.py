@@ -44,6 +44,8 @@ def lib():
     L.gp_destroy.restype = None
     L.gp_last_error.argtypes = [c_void_p]
     L.gp_last_error.restype = c_char_p
+    L.gp_last_call_error.argtypes = []
+    L.gp_last_call_error.restype = c_char_p
     L.gp_load_tensor.argtypes = [c_void_p, c_char_p, c_void_p, c_int, POINTER(c_int64), c_int]
     L.gp_set_text_embed.argtypes = [c_void_p, c_void_p, c_int, c_int]
     L.gp_encode_text.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p]
@@ -109,8 +111,6 @@ def lib():
     L.gp_resize_pil.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p]
     L.gp_jpeg_probe.argtypes = [c_char_p, c_size_t, POINTER(c_int), POINTER(c_int), POINTER(c_int64)]
     L.gp_jpeg_decode.argtypes = [c_char_p, c_size_t, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p]
-    L.gp_jpeg_last_error.argtypes = []
-    L.gp_jpeg_last_error.restype = c_char_p
     L.gp_v1_postprocess.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p]
     L.gp_depth_align.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
@@ -139,9 +139,20 @@ def _rgb_arg(rgb):
     return (rgb.float() if rgb.dtype == torch.bfloat16 else rgb).contiguous()
 
 
+def _error_text(what, st, msg):
+    """The text of an exception for status `st` of C-ABI call `what`, with the library's reason `msg`."""
+    return f"{what}: {_STATUS.get(st, st)}: {msg}"
+
+
+def _call_error():
+    """The library's reason for this thread's last failed call that takes no engine (gp_last_call_error)."""
+    return lib().gp_last_call_error().decode()
+
+
 def _check_free(st, what):
+    """Raises RuntimeError for a failed C-ABI call that takes no engine."""
     if st != 0:
-        raise RuntimeError(f"{what} failed: {_STATUS.get(st, st)} (see stderr)")
+        raise RuntimeError(_error_text(what, st, _call_error()))
 
 
 class Engine:
@@ -161,9 +172,7 @@ class Engine:
         self.precision = precision
         self.arch = arch
         self.h = c_void_p()
-        st = self.L.gp_create(byref(cfg), byref(self.h))
-        if st != 0:
-            raise RuntimeError(f"gp_create failed: {_STATUS.get(st, st)} (no sm_90a device?)")
+        _check_free(self.L.gp_create(byref(cfg), byref(self.h)), "gp_create")
         self.plan_shape = None
         self.out_hw = None
         self.memory_efficient_attention = False
@@ -205,8 +214,7 @@ class Engine:
 
     def _ck(self, st, what):
         if st != 0:
-            msg = self.L.gp_last_error(self.h).decode()
-            raise RuntimeError(f"{what}: {_STATUS.get(st, st)}: {msg}")
+            raise RuntimeError(_error_text(what, st, self.L.gp_last_error(self.h).decode()))
 
     def load_state(self, component, sd):
         """component in {unet, vae, dpt}: sd = {diffusers key: tensor}; or "text": sd = transformers' CLIPTextModel
@@ -758,8 +766,9 @@ def jpeg_probe(data):
     stream; ``ValueError`` with the reason otherwise."""
     data = bytes(data)
     H, W, ws = c_int(), c_int(), c_int64()
-    if lib().gp_jpeg_probe(data, len(data), byref(H), byref(W), byref(ws)) != 0:
-        raise ValueError(f"JPEG not taken by the GPU decoder: {lib().gp_jpeg_last_error().decode()}")
+    st = lib().gp_jpeg_probe(data, len(data), byref(H), byref(W), byref(ws))
+    if st != 0:
+        raise ValueError(_error_text("gp_jpeg_probe", st, _call_error()))
     return H.value, W.value, ws.value
 
 
@@ -785,7 +794,7 @@ def decode_jpeg(data, device=None, layout="chw"):
         st = lib().gp_jpeg_decode(data, len(data), c_void_p(ws.data_ptr()), ws_bytes, c_void_p(out.data_ptr()),
                                   *strides, _stream_ptr(dev))
     if st == 1:
-        raise ValueError(f"GPU JPEG decode failed: {lib().gp_jpeg_last_error().decode()}")
+        raise ValueError(_error_text("gp_jpeg_decode", st, _call_error()))
     _check_free(st, "gp_jpeg_decode")
     return out
 

@@ -59,7 +59,11 @@ typedef struct {
 /* replaces: GenPerceptPipeline.__init__/from_pretrained model assembly (run.py:314-376) */
 gp_status gp_create(const gp_config* cfg, gp_engine** out);
 void gp_destroy(gp_engine* e);
+/* the reason of engine `e`'s last failed call */
 const char* gp_last_error(gp_engine* e);
+/* the reason of the calling thread's last failed call that takes no engine (gp_create, the per-kernel, pre/post,
+ * evaluation, JPEG, shared-arena and host-only query entry points), or "" when the last such call succeeded */
+const char* gp_last_call_error(void);
 
 /* replaces: load_state_dict of the diffusers-format checkpoints (run.py:336-357, :296-312).
  * `key` = "<component>.<diffusers key>", component in {unet, vae, dpt}, or "text" (gp_encode_text).  Host pointer, copied. */
@@ -319,7 +323,7 @@ gp_status gp_resize_pil(const uint8_t* src_hwc, int src_on_host, int H, int W, u
  * components libjpeg infers as YCbCr (JFIF, Adobe transform 1, or ids 1-2-3), one interleaved scan, luma sampling
  * 1x1, 2x1 or 2x2 with 1x1 chroma, any restart interval.  Everything else is GP_ERR_INVALID.
  * gp_jpeg_probe is host only (no device needed): GP_OK with the frame size and the workspace the decode needs, or
- * GP_ERR_INVALID with the reason in gp_jpeg_last_error().
+ * GP_ERR_INVALID with the reason in gp_last_call_error().
  * gp_jpeg_decode uploads the file bytes into the caller's device workspace (>= the probed size; nothing is allocated),
  * decodes on `stream` and writes dst[y * row_stride + x * pixel_stride + c * channel_stride] (uint8, device; strides
  * in elements), then waits for the status word: GP_ERR_INVALID for a stream that is corrupt, whose markers are not
@@ -328,8 +332,6 @@ gp_status gp_jpeg_probe(const uint8_t* data, size_t nbytes, int* H, int* W, int6
 gp_status gp_jpeg_decode(const uint8_t* data_host, size_t nbytes, void* workspace_dev, int64_t workspace_bytes,
                          uint8_t* dst_dev, int64_t row_stride, int64_t pixel_stride, int64_t channel_stride,
                          void* stream);
-/* the reason of the calling thread's last gp_jpeg_probe / gp_jpeg_decode failure ("" after a success) */
-const char* gp_jpeg_last_error(void);
 /* replaces: the post-processing of GenPercept v1's __call__ (GenPercept_v1/genpercept/pipeline_genpercept.py) on the
  * engine's map.  pred: fp32 [B,C,h,w] in [0,1] on the device (gp_infer's out); p = 2 pred - 1 is v1's single_infer result.
  * p is taken to (H, W) by F.interpolate (task 0 / 1: bilinear, align_corners=False, no antialiasing; task 2: the legacy
